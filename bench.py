@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Benchmark: Dreamer-V3 train-steps/sec (BASELINE.json metric) on N B200s.
+"""Benchmark: Dreamer-V3 train-steps/sec (BASELINE.json metric) on N H100s.
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA engine
     python bench.py --impl reference --steps K --warmup W    # reference algorithm on the host cores (oracle port)
+    python bench.py --steps K --dump-outputs DIR              # also write the last timed step's results as DIR/*.npy
 
 One "step" = one call of the Dreamer-V3 update (`train()`, reference dreamer_v3.py:48-357) on one per-rank
 replay batch of the BASELINE config: size S, B=16, T=64, 64x64x3 uint8 observations, horizon 15, discrete A=2.
@@ -41,7 +42,7 @@ def workload_config(args):
     """identical in both arms (`--impl b200` / `--impl reference`)"""
     return {"workload": workload_name(args), "size": args.size, "per_rank_batch": args.batch, "seq_len": args.seq,
             "horizon": args.horizon,
-            "l2": "per-step working set (activations + optimiser state, GBs) >> 126 MB L2: no flush needed between steps"}
+            "l2": "per-step working set (activations + optimiser state, GBs) >> 50 MB L2: no flush needed between steps"}
 
 
 def make_cfg(args, **over):
@@ -56,8 +57,8 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), "measured"
-    return 6650.0, 1590.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops", 989.0), "measured"
+    return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 class ClockSampler:
@@ -284,6 +285,8 @@ def run_b200(args):
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(eng, args.dump_outputs)
     # ---- timed region 2: `e2e`: the same public call with the batch in pinned HOST memory (H2D inside train()) and
     # a device->host read of the step's 13 metrics
     e2, e3 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -328,10 +331,10 @@ def run_b200(args):
     value = world * args.steps / (ms / 1e3)
     e2e_v = world * args.steps / (ms_e2e / 1e3)
     hbm, tf, src = measured_peaks()
-    # Dominant kernel: gemm_tc_kernel (tcgen05 3xTF32; serves every large Linear / conv forward, input-gradient
+    # Dominant kernel: gemm_tc_kernel (wgmma 3xTF32; serves every large Linear / conv forward, input-gradient
     # and weight-gradient product).  `achieved` = algorithmic FLOPs of its largest launch in the step (an MLP
     # GEMM over the imagined trajectories: M=(H+1)*T*B, N=dense_units, K=latent) / its mean launch duration, measured
-    # here with CUDA events on the launching stream; operands exceed the 126 MB L2.
+    # here with CUDA events on the launching stream.
     tot_ms = sum(v[0] for v in breakdown.values()) or 1.0
     tc_ops = ("gemm", "gemm_ln_act", "gemm_ln_gru", "conv_down", "conv_up", "conv_wgrad")
     share = sum(breakdown[k][0] for k in tc_ops if k in breakdown) / tot_ms
@@ -350,16 +353,9 @@ def run_b200(args):
     torch.cuda.synchronize()
     g_ms = g0.elapsed_time(g1) / 20
     g_tf = 2.0 * gm * gn * gk / (g_ms * 1e-3) / 1e12
-    traffic, tsrc = None, None
-    for name in ("r2_gemm_tc_traffic.json", "r1_gemm_tc_traffic.json"):
-        tpath = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(tpath) and args.size == "S":
-            traffic, tsrc = json.load(open(tpath)).get("dram_bytes_per_launch"), name
-            break
     flops_step = {"S": 0.904e12, "XL": 37.6e12}.get(args.size) if (args.batch, args.seq, args.horizon) in ((16, 64, 15), (64, 64, 15)) else None
-    roof = {"kernel": "gemm_tc_kernel<128> (tcgen05.mma kind::tf32, 3xTF32 split, TMA, TMEM)", "bound": "tensor",
-            "achieved": g_tf, "peak": tf, "unit": "TFLOP/s", "frac": g_tf / tf, "traffic": traffic,
-            "traffic_source": tsrc, "peak_source": f"{src} bf16 cuBLAS",
+    roof = {"kernel": "gemm_tc_kernel<128> (wgmma.mma_async tf32, 3xTF32 split, TMA)", "bound": "tensor",
+            "achieved": g_tf, "peak": tf, "unit": "TFLOP/s", "frac": g_tf / tf, "peak_source": f"{src} bf16 dense",
             "shape": {"M": gm, "N": gn, "K": gk}, "us_per_launch": g_ms * 1e3,
             "step_tflops": (flops_step * world / (ms / args.steps * 1e-3) / 1e12 / world) if flops_step else None,
             "step_frac_of_peak": (flops_step / (ms / args.steps * 1e-3) / 1e12 / tf) if flops_step else None,
@@ -396,12 +392,12 @@ def run_b200(args):
 
 # ---------------------------------------------------------------------------------------------------------
 # Baseline arms: the reference algorithm on the host cores / in torch eager on the same GPU.
-# `kind: "reference"` = the UNMODIFIED reference train() (package installed into baseline/_ref by __graft_entry__.build(),
+# `kind: "reference"` = the UNMODIFIED reference train() (package copied into oracle/_ref by __graft_entry__.build(),
 # imported through the stub harness oracle/ref_harness.py); `kind: "port"` = oracle/dv3_oracle.py when no reference tree is
 # reachable.  Only these arms execute anything under oracle/.
 # ---------------------------------------------------------------------------------------------------------
 def reference_root():
-    for p in (os.environ.get("SHEEPRL_REFERENCE_ROOT"), os.path.join(ROOT, "baseline", "_ref"), "/root/reference"):
+    for p in (os.environ.get("SHEEPRL_REFERENCE_ROOT"), os.path.join(ROOT, "oracle", "_ref")):
         if p and os.path.isdir(os.path.join(p, "sheeprl")):
             return p
     return None
@@ -521,7 +517,7 @@ def cpu_baseline(args, steps: int, warmup: int):
     return {"value": len(tt) / sum(tt), "unit": UNIT, "cores": best_k, "kind": kind,
             "sample": f"{len(tt)} full train() step(s) of the same workload after {warmup} warm-up, torch fp32 CPU, "
                       f"{best_k} of {cores} host threads; s/step={sum(tt) / len(tt):.2f}; "
-                      + ("the UNMODIFIED reference (baseline/_ref) through the stub-import harness" if kind == "reference"
+                      + ("the UNMODIFIED reference (oracle/_ref) through the stub-import harness" if kind == "reference"
                          else "oracle port of the reference (no reference tree on this host)")}
 
 
@@ -569,6 +565,27 @@ def run_reference(args):
     print(json.dumps(out))
 
 
+def dump_outputs(eng, out_dir, max_per_group=4 << 20):
+    """What the timed train() call leaves to its caller after its last step: the step's losses / gradient norms and the
+    updated world-model, actor and critic parameters.  A group larger than `max_per_group` floats is written as a fixed
+    sample of its flat buffer (the sorted first `max_per_group` entries of a seed-0 permutation), so the files stay below
+    64 MB in all."""
+    import numpy as np
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, "metrics.npy"), eng.metrics.detach().cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "norms.npy"), eng.norms.detach().cpu().numpy().astype(np.float32))
+    for name in ("wm", "actor", "critic"):
+        flat = getattr(eng, name).flat.detach()
+        if flat.numel() > max_per_group:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(flat.numel(), generator=g)[:max_per_group].sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(out_dir, f"{name}.npy"), flat.cpu().numpy().astype(np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -587,6 +604,8 @@ def main():
     ap.add_argument("--no-overlap-allreduce", action="store_true", help="one all-reduce of the whole world-model gradient "
                     "before the optimizer instead of three overlapped buckets (the default when the persistent scan runs)")
     ap.add_argument("--overlap-allreduce", action="store_true", help="force the three overlapped bucket reductions")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="after the timed steps, write the last step's "
+                    "metrics, gradient norms and (sampled) updated parameters as DIR/<name>.npy")
     args = ap.parse_args()
     if args.batch is None:
         args.batch = 16 if args.size == "S" else 64

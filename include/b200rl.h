@@ -1,4 +1,4 @@
-/* b200rl — C-ABI of the B200 (sm_100a) kernels behind SheepRL's Dreamer-V3 / PPO / SAC update paths.
+/* b200rl — C-ABI of the H100 (sm_90a) kernels behind SheepRL's Dreamer-V3 / PPO / SAC update paths.
  *
  * The reference (Eclectic-Sheep/sheeprl) is pure Python and has NO native interface for this path
  * (SURVEY.md §0 F1, §2.2); these entry points are what a reference-side binding (ctypes / a
@@ -11,7 +11,7 @@
  *     `stream` (pass the caller's current stream) — hence CUDA-graph capturable;
  *   - fp32, row-major; `ld*` = row stride in elements of a 2-D view whose inner stride is 1;
  *   - return 0 on success; non-zero => b200rl_last_error() (thread-local message);
- *   - built for sm_100a only (b200rl_device_check refuses other devices). There is no CPU fallback.
+ *   - built for sm_90a only (b200rl_device_check refuses other devices). There is no CPU fallback.
  */
 #ifndef B200RL_H_
 #define B200RL_H_
@@ -34,7 +34,7 @@ int b200rl_device_check(void);
 int b200rl_gemm_f32(const float* A, const float* B, float* C, const float* bias, int M, int N, int K, int lda, int ldb,
                     int ldc, int transA, int transB, int accumulate, cudaStream_t stream);
 /* Tensor-core path used by b200rl_gemm_f32 for large NT products (transA = 0, transB = 1, 16-byte aligned
- * operands): 3xTF32 split-precision on tcgen05.mma with TMA-fed 128B-swizzled tiles and TMEM accumulators
+ * operands): 3xTF32 split-precision on wgmma.mma_async with TMA-fed 128B-swizzled tiles and register accumulators
  * (gemm_tc.cu).  Same contract as b200rl_gemm_f32; `_supported` tells whether a shape is eligible. */
 /* Precision of every tensor-core product (GEMM, conv forward / input gradient / weight gradient), process-wide like
  * torch.set_float32_matmul_precision (the reference sets it from configs/config.yaml:18, default "high"):
@@ -47,7 +47,7 @@ int b200rl_gemm_tc_supported(const float* A, const float* B, int M, int N, int K
 int b200rl_gemm_tc(const float* A, const float* B, float* C, const float* bias, int M, int N, int K, int lda, int ldb,
                    int ldc, int transA, int transB, int accumulate, cudaStream_t stream);
 /* Dense block Linear(bias=False) -> LayerNorm(eps) -> activation in two launches (sheeprl/utils/model.py:34-88 miniblock,
- * as built by MLP at sheeprl/models/models.py:23-119): the tcgen05 product leaves split-K partial tiles, one kernel sums
+ * as built by MLP at sheeprl/models/models.py:23-119): the wgmma product leaves split-K partial tiles, one kernel sums
  * them in split order, normalises the row in registers and applies the activation.  `pre` (optional) keeps W.x for the
  * backward.  mode 1 (N = 3R): the tail is LayerNormGRUCell's gate instead (sheeprl/models/models.py:396-403): h_out (and
  * h_out2, optional second copy, e.g. the next step's [h | x] input) = u * tanh(r * c) + (1 - u) * h_prev; `out` (optional)
@@ -85,7 +85,7 @@ int b200rl_conv_up(const float* small_, const float* W, float* big, const float*
 int b200rl_conv_wgrad(const float* small_, const float* big, float* dW, int NB, int h, int w, int Cs, int Cb,
                       int accumulate, cudaStream_t stream);
 /* Tensor-core implicit-GEMM versions of conv_down / conv_up (gemm_tc.cu: 4-D TMA boxes gather the taps, no
- * im2col buffer, 3xTF32 tcgen05).  `Wpacked` is a caller-owned 16*Cs*Cb-float workspace filled by
+ * im2col buffer, 3xTF32 wgmma).  `Wpacked` is a caller-owned 16*Cs*Cb-float workspace filled by
  * b200rl_conv_pack (down: [Cs][tap][Cb]; up: [parity][Cb][tap][Cs]) after every weight update.  Eligible when the
  * gathered image has a multiple of 32 channels and the small grid tiles by 128 pixels (`_supported`). */
 /* Weight gradient as one tensor-core GEMM over all pixels: small^T [Cs][P] times the transposed im2col of `big`
@@ -317,7 +317,7 @@ int b200rl_lambda_returns_bwd(const float* cont_logit, const float* discount, co
 int b200rl_twohot_mean_bwd(const float* logits, const float* d_mean, float* d_logits, long long M, int nb, long long ldl,
                            long long ldd, float low, float high, cudaStream_t stream);
 
-/* Convolution weight gradient with both operands read in place as MN-major tcgen05 operands (no im2col, no transposes):
+/* Convolution weight gradient with both operands read in place as MN-major tiles (no im2col, no transposes):
  * G[(tap, cb), cs] = sum over small pixels p of big[patch(p)][tap][cb] * small[p][cs]; big [NB,2h,2w,Cb] and small
  * [NB,h,w,Cs] channel-last, G [16*Cb][Cs] (unpacked to the reference's [Cs][Cb][4][4] by b200rl_conv_wgrad_tc).
  * Replaces the autograd weight-gradient of CNNEncoder / CNNDecoder convolutions (agent.py:78-91, :199-222). */

@@ -1,11 +1,11 @@
-"""TEST INFRASTRUCTURE — container-only import harness for the REAL reference.
+"""TEST INFRASTRUCTURE — import harness for the REAL reference.
 
-Imports the unmodified reference package from /root/reference (read-only, not present on the
-GPU box) with permissive stubs for the third-party packages that are absent in this image
-(lightning, hydra, omegaconf, gymnasium, torchmetrics, ...).  It is used ONLY to
-  * pin oracle/dv3_oracle.py against the executed reference (tests/test_oracle_pin.py,
-    skipped when /root/reference is absent), and
-  * generate the committed golden fixtures (oracle/make_golden.py -> tests/golden/).
+Imports the unmodified reference package from $SHEEPRL_REFERENCE_ROOT, else from oracle/_ref (placed there by
+oracle/install_ref.py during build(); absent where no reference checkout was available) with permissive stubs for
+the third-party packages this project does not depend on (lightning, hydra, omegaconf, gymnasium, torchmetrics, ...).
+It is used ONLY to
+  * run the tests that execute the reference itself (skipped when it is absent), and
+  * generate the committed golden fixtures (oracle/make_golden*.py -> tests/golden/).
 Nothing in the product package imports this module.
 
 Recipe follows SURVEY.md Appendix C.
@@ -19,7 +19,8 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("SHEEPRL_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("SHEEPRL_REFERENCE_ROOT",
+                                os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref"))
 _STUB_ROOTS = {
     "lightning", "hydra", "omegaconf", "gymnasium", "torchmetrics", "moviepy",
     "lightning_utilities", "pytorch_lightning", "mlflow", "pygame", "dotenv_stub_never",

@@ -1,8 +1,8 @@
-"""Builds the in-tree CUDA library `sheeprl_b200/libb200rl.so` for sm_100a with nvcc.
+"""Builds the in-tree CUDA library `sheeprl_b200/libb200rl.so` for sm_90a (H100) with nvcc.
 
     python -m sheeprl_b200.build [--force]
 
-nvcc cross-compiles without a GPU; the .so is git-ignored but travels to the GPU box with the tree.
+nvcc cross-compiles without a GPU; the .so and the objects under `_build/` are build products (git-ignored).
 """
 from __future__ import annotations
 
@@ -16,7 +16,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "_build")
 LIB = os.path.join(HERE, "libb200rl.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-diag-suppress", "177"]
 
 

@@ -17,8 +17,8 @@ extern "C" const char* b200rl_last_error(void) { return g_err; }
 
 extern "C" int b200rl_abi_version(void) { return 1; }
 
-// Compiled-for architecture, so the loader can refuse anything but sm_100a.
-extern "C" const char* b200rl_build_arch(void) { return "sm_100a"; }
+// Compiled-for architecture, so the loader can refuse anything but sm_90a.
+extern "C" const char* b200rl_build_arch(void) { return "sm_90a"; }
 
 extern "C" int b200rl_device_check(void) {
   int dev = 0;
@@ -27,8 +27,8 @@ extern "C" int b200rl_device_check(void) {
     b200rl_set_error("no CUDA device");
     return B200RL_ERR_CUDA;
   }
-  if (prop.major != 10) {
-    b200rl_set_error("b200rl is built for sm_100a only; found sm_%d%d", prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    b200rl_set_error("b200rl is built for sm_90a only; found sm_%d%d", prop.major, prop.minor);
     return B200RL_ERR_CUDA;
   }
   return B200RL_OK;

@@ -1,4 +1,4 @@
-// Shared helpers for the b200rl CUDA library (sm_100a only).
+// Shared helpers for the b200rl CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -37,7 +37,7 @@ extern "C" void b200rl_set_error(const char* fmt, ...);
   } while (0)
 
 static constexpr float kFp32Eps = 1.1920928955078125e-07f;
-static constexpr int kNumSMs = 148;
+static constexpr int kNumSMs = 132;   // H100 SXM
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll

@@ -503,7 +503,7 @@ extern "C" int b200rl_conv_wgrad_tc(const float* small_, const float* big, float
   const long long P = (long long)NB * h * w, Pp = (P + 3) / 4 * 4;
   RL_CHECK_ARG(P >= 1024 && Cs >= 48 && Cb >= 8 && P <= 2000000000LL, "shape not eligible for the tensor-core wgrad path");
   if (b200rl_conv_wgrad_mn_supported(NB, h, w, Cs, Cb)) {
-    // operands read in place: the gathered big image and the small image are both MN-major tcgen05 operands
+    // operands read in place: the gathered big image and the small image are both MN-major tiles
     float* G = workspace;                      // [16*Cb][Cs]
     if (int rc = b200rl_conv_wgrad_mn(small_, big, G, NB, h, w, Cs, Cb, st)) return rc;
     wgrad_unpack_kernel<<<ceil_div(16LL * Cs * Cb, 256), 256, 0, st>>>(G, dW, Cs, Cb, accumulate);

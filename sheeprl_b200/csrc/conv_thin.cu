@@ -4,7 +4,7 @@
 // With CB = 3 these are not tensor-core shapes (K or N of 3..48) and they move the two largest activations of the
 // model (1024 x 32x32x32 fp32 = 134 MB and the 50 MB image), so they are written as FMA/LDS-balanced SIMT kernels
 // that read every activation once with full 128-byte lines:
-//   bound: max(HBM: 184 MB / launch, FMA: 1.6 GFMA / launch) ~ 50-60 us on a B200; the generic implicit-GEMM kernels
+//   bound: max(HBM: 184 MB / launch, FMA: 1.6 GFMA / launch) (not measured on the H100); the generic implicit-GEMM kernels
 //   they replace took 1.5 ms (up) and 0.7 ms (wgrad) per launch.
 // Weights keep the reference layout W[Cs][CB][ky][kx] (see conv.cu header for the index conventions).
 #include "common.cuh"
@@ -215,20 +215,22 @@ conv_wgrad_thin_kernel(const float* __restrict__ small, const float* __restrict_
 
 
 // ---------------------------------------------------------------------------------------------------------
-// Packed-FMA (FFMA2, fma.rn.f32x2) versions for 32-wide small grids (the 64x64 images of Dreamer-V3): one warp per pair of
-// small-grid rows, lane = column.  The generic kernels above issue ~4 instructions per FMA (ncu r2_thin_convs: IPC 3.2 of
-// 4 with the FMA pipe 43 % busy — issue bound); here every weight LDS.128 (warp-uniform, one wavefront) feeds 4-8 packed
-// FMAs and the image rows are staged once per warp in shared memory in a conflict-free layout.
+// Paired-FMA versions for 32-wide small grids (the 64x64 images of Dreamer-V3): one warp per pair of small-grid rows,
+// lane = column.  The generic kernels above issue ~4 instructions per FMA; here every weight LDS.128 (warp-uniform, one
+// wavefront) feeds 8-16 FMAs on 64-bit register pairs and the image rows are staged once per warp in shared memory in a
+// conflict-free layout.
 // ---------------------------------------------------------------------------------------------------------
 typedef unsigned long long u64;
-__device__ __forceinline__ void fma2(u64& acc, u64 x, u64 w) { asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(x), "l"(w)); }
-__device__ __forceinline__ u64 dup2(float x) {
-  u64 r;
-  asm("mov.b64 %0, {%1, %1};" : "=l"(r) : "r"(__float_as_uint(x)));
-  return r;
-}
 __device__ __forceinline__ float lo32(u64 v) { return __uint_as_float((unsigned)v); }
 __device__ __forceinline__ float hi32(u64 v) { return __uint_as_float((unsigned)(v >> 32)); }
+__device__ __forceinline__ u64 pack2(float lo, float hi) {
+  return ((u64)__float_as_uint(hi) << 32) | (u64)__float_as_uint(lo);
+}
+// two independent round-to-nearest FMAs on the halves of a register pair
+__device__ __forceinline__ void fma2(u64& acc, u64 x, u64 w) {
+  acc = pack2(fmaf(lo32(x), lo32(w), lo32(acc)), fmaf(hi32(x), hi32(w), hi32(acc)));
+}
+__device__ __forceinline__ u64 dup2(float x) { return pack2(x, x); }
 
 // down_thin: Conv2d(3 -> CS, k4 s2 p1) on [NB][2h][64][3] -> [NB][h][32][CS]  (CNNEncoder first layer, agent.py:78-91; also
 // the input-gradient pass of the decoder's last ConvTranspose2d).  A warp owns two output rows (64 pixels) x 32 channels.

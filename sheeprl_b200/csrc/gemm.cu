@@ -1,9 +1,9 @@
 // fp32 SIMT GEMM family: C[M,N] = op(A) * op(B) (+bias) (+C)
 //
 // This is the exact-fp32 (FFMA) path used for (a) the latency-bound skinny GEMMs of the RSSM scan
-// (M = batch 16) and (b) every shape the tensor-core path (gemm_tc.cu, 3xTF32 tcgen05) does not take.
+// (M = batch 16) and (b) every shape the tensor-core path (gemm_tc.cu, 3xTF32 wgmma) does not take.
 // Register-blocked, shared-memory tiled, register-prefetch double buffered, optional split-K
-// (fp32 atomics) so that weight-gradient GEMMs (tiny output, reduction over T*B rows) fill 148 SMs.
+// (fp32 atomics) so that weight-gradient GEMMs (tiny output, reduction over T*B rows) fill the SMs.
 //
 // Reference ops replaced: nn.Linear forward / its autograd backward as used throughout
 // sheeprl/algos/dreamer_v3/agent.py (MLP, RecurrentModel, representation/transition models).
@@ -213,7 +213,7 @@ rank_k_nn_kernel(const float* __restrict__ A, const float* __restrict__ B, float
   *out = acc;
 }
 
-// include/b200rl.h: b200rl_gemm_f32.  Large NT products go to the tcgen05 3xTF32 kernel (gemm_tc.cu); everything
+// include/b200rl.h: b200rl_gemm_f32.  Large NT products go to the wgmma 3xTF32 kernel (gemm_tc.cu); everything
 // else (skinny, transposed, unaligned) runs on the exact-fp32 FFMA kernels below.
 extern "C" int b200rl_gemm_f32(const float* A, const float* B, float* C, const float* bias, int M, int N, int K,
                                int lda, int ldb, int ldc, int transA, int transB, int accumulate,

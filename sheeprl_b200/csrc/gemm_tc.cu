@@ -1,26 +1,22 @@
-// Tensor-core GEMM for sm_100a: C[M,N] = A[M,K] * B[N,K]^T (+bias) (+C), fp32 in / fp32 out, computed as
-// 3xTF32 on the 5th-generation tensor cores (tcgen05.mma kind::tf32, accumulators in TMEM, operands staged
-// in shared memory by TMA with the 128-byte swizzle).
+// Tensor-core GEMM for sm_90a: C[M,N] = A[M,K] * B[N,K]^T (+bias) (+C), fp32 in / fp32 out, computed as 3xTF32 on the
+// Hopper tensor cores (wgmma.mma_async kind tf32, operands staged in shared memory by TMA with the 128-byte swizzle,
+// stages handed over with mbarriers).
 //
 // Why 3xTF32: the parity bar for this path is 1e-4 against an fp32 CPU oracle through chains of ~100 dependent
 // layers (SURVEY.md §0 F7).  Each fp32 operand x is split in-kernel into hi = x with the 13 low mantissa bits
 // cleared (exactly what the TF32 datapath keeps) and lo = x - hi (exact in fp32); the product is accumulated
 // as hi*hi + hi*lo + lo*hi in fp32 (the dropped lo*lo term is ~2^-22 relative).  Effective rate is 1/3 of the
-// TF32 peak, ~10x the FFMA path.
+// TF32 peak.
 //
-// Pipeline (per 128x128 output tile, K step 32 = one 128-byte swizzle atom):
-//   warp 0   : TMA producer   -- cp.async.bulk.tensor loads of the raw fp32 A / B tiles, mbarrier complete_tx
-//   warps 4-7: splitters      -- write `lo` = x - trunc_tf32(x) of each landed tile to a twin buffer (same swizzled
-//                                offsets, so the split is layout-agnostic), fence.proxy.async, arrive.  The raw tile
-//                                itself serves as `hi`: the TF32 datapath ignores the 13 low mantissa bits (measured:
-//                                identical 1.2e-6 error, 130 -> 151 TF/s from not re-writing hi: the kernel is
-//                                shared-memory-bandwidth bound, 160 KB of smem traffic per 128x128x32 k-block)
-//   warp 1   : MMA issuer     -- one elected lane issues 4 k-steps x 3 tcgen05.mma per stage, tcgen05.commit
-//                                releases the stage back to the producer
-//   warps 8-15: accumulators  -- every 4 k-blocks tcgen05.ld the finished TMEM chunk and add it into fp32
-//                                registers with RN adds (the tensor core accumulates with truncation), double
-//                                buffered TMEM; finally +bias / +C and store
-//   warp 2   : TMEM allocator
+// Pipeline (per 128 x BN output tile, K step 32 = one 128-byte swizzle atom), 384 threads = three warpgroups:
+//   warp 0    : TMA producer   -- cp.async.bulk.tensor loads of the raw fp32 A / B tiles, mbarrier complete_tx
+//   warps 1-3 : B splitters    -- write hi = trunc_tf32(x) and lo = x - hi of each landed B tile to two K-major
+//                                 128B-swizzled buffers (wgmma reads tf32 B only K-major from shared memory, so an
+//                                 MN-major B tile is transposed on the way), fence.proxy.async, arrive
+//   warpgroups 1, 2: consumers -- rows [0, 64) / [64, 128) of the tile: load their A fragment straight from the raw
+//                                 swizzled tile into registers (any layout, split in registers), issue 4 k-steps x 3
+//                                 wgmma per stage, and every CH stages add the finished chunk accumulator into fp32
+//                                 registers with RN adds; finally +bias / +C and store
 // Replaces: every large nn.Linear forward / input-gradient product of the Dreamer-V3 step
 // (sheeprl/models/models.py MLP; agent.py heads, RSSM imagination, actor, critic).
 //
@@ -40,15 +36,15 @@
 
 namespace {
 
-constexpr int BM = 128, BK = 32, STAGES = 4;   // 4 x 48 KB operand stages; TMEM: 2 accumulators + 4 x (A hi | lo) = 512 columns
-// 18 warps: 0 TMA, 1 MMA, 4-7 split A (-> TMEM), 8-15 accumulate, {2, 3, 16, 17} split B (-> shared memory; warp 2 also
-// owns the TMEM allocation).  A and B of a stage are split concurrently by different warps: the hi/lo split is a chain
-// of dependent latencies (barrier -> LDS -> ALU -> tcgen05.st / STS -> fence), the longest stage of the pipeline for the
-// convolutions' narrow N tiles.
-constexpr int NTHREADS = 576;
-constexpr int SPLIT_WARP0 = 4, NSPLIT_THREADS = 128;
-constexpr int ACC_WARP0 = 8, NACC_WARPS = 8;
-constexpr int BSPLIT_WARP_HI = 16;                  // B splitters: warps 2, 3, 16, 17
+constexpr int BM = 128, BK = 32;
+constexpr int NTHREADS = 384;
+constexpr int NSPLIT_THREADS = 96;                  // warps 1-3
+constexpr int NCONS_WARPS = 8;                      // warpgroups 1 and 2
+// register budget per thread after setmaxnreg: the producer warpgroup gives its registers to the consumers, which hold
+// the chunk accumulator, the running fp32 sum and the A fragments of a stage (128 x BN tile: up to 64 + 64 + 32)
+constexpr int PRODUCER_REGS = 56, CONSUMER_REGS = 224;
+// operand stages that fit the 227 KB of shared memory: raw A, raw B, B hi, B lo per stage
+template <int BN> constexpr int stages_for() { return BN == 128 ? 3 : 5; }
 
 // ---------------------------------------------------------------- PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -110,116 +106,82 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
       "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// A operand from tensor memory (lane = tile row, one 32-bit column per k element), B from a shared-memory descriptor
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_c, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                             uint32_t accumulate) {
+
+// D[64 x N] (+)= A[64 x 8] (registers, tf32) * B[N x 8]^T (shared memory descriptor, K-major); scale_d = 0 overwrites D
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, int scale_d) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t"
-      "}" ::"r"(tmem_c),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\twgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
+__device__ __forceinline__ void wgmma_tf32(float (&d)[64], const uint32_t (&a)[4], uint64_t desc_b, int scale_d) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\twgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// Pins registers an in-flight wgmma reads or writes: the compiler may neither move their uses across this point nor
+// reuse them before it.
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+template <int N, int W>
+__device__ __forceinline__ void fence_regs(uint32_t (&r)[N][W]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i)
+#pragma unroll
+    for (int j = 0; j < W; ++j) asm volatile("" : "+r"(r[i][j])::"memory");
 }
 
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// K-major operand tile [rows][32 fp32] with 128B swizzle: 8-row groups are 1024 B apart (SBO), one atom along K.
+// K-major operand tile [rows][32 fp32] with the 128B swizzle: 8-row groups are 1024 B apart (SBO); a k-step of 8 tf32
+// advances the start address by 32 B inside the swizzle row.  Layout type 1 = SWIZZLE_128B (bits 62-63).
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);       // start address, bits [0,14)
-  d |= (uint64_t)0 << 16;                            // leading byte offset (unused: single atom along K)
+  d |= (uint64_t)1 << 16;                            // leading byte offset (unused: a k-step stays inside one atom)
   d |= (uint64_t)(1024 >> 4) << 32;                  // stride byte offset between 8-row groups
-  d |= (uint64_t)1 << 46;                            // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                            // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                            // SWIZZLE_128B
   return d;
 }
 
-// MN-major operand tile (the operand is stored [K][MN] in global memory: transposed products without transposes).
-// For 32-bit (tf32) operands the only MN-major shared-memory layout the tensor core accepts is the 128-byte swizzle
-// with a 32-byte base (CUTLASS: Layout_MN_SW128_32B_Atom, TMA: CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B): atoms of 4 k-rows x
-// 128 B (32 MN floats) in which the 32-byte chunk index is XOR-ed with the row index.  A TMA box {32 MN floats, 32
-// k-rows} lands as eight such atoms (4 KB); a 128-wide tile is four of those blocks.  Descriptor: LBO = distance
-// between 32-wide MN blocks (4096 B), SBO = distance between 4-row k atoms (512 B); one K=8 instruction reads two atoms.
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(4096 >> 4) << 16;                  // leading byte offset: next 32-element MN block
-  d |= (uint64_t)(512 >> 4) << 32;                   // stride byte offset: next 4-row k atom
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)1 << 61;                            // SWIZZLE_128B_BASE32B
-  return d;
+// Byte offsets of element (r, k) in the two raw tile layouts TMA writes with the 128-byte swizzle (16-byte chunk index
+// XOR-ed with the 128-byte line index):
+//   K-major  [rows][32 k]              : line = row
+//   MN-major [rows / 32][32 k][32 rows]: 4 KB per 32-row block (one TMA box), line = k
+__device__ __forceinline__ uint32_t kmajor_off(int r, int k) {
+  return (uint32_t)(r * 128 + ((((k >> 2) ^ r) & 7) << 4) + (k & 3) * 4);
+}
+__device__ __forceinline__ uint32_t mnmajor_off(int r, int k) {
+  return (uint32_t)((r >> 5) * 4096 + k * 128 + (((((r & 31) >> 2) ^ k) & 7) << 4) + (r & 3) * 4);
 }
 
 template <int BN>
 struct Smem {
+  static constexpr int STAGES = stages_for<BN>();
   // every operand buffer is a whole number of 1024-byte swizzle groups
-  float a_hi[STAGES][BM * BK];   // raw A tiles; their hi / lo halves go to TENSOR MEMORY (see kATmem below)
-  float b_hi[STAGES][BN * BK];
+  float a[STAGES][BM * BK];      // raw A tiles (the consumers split them in registers)
+  float b[STAGES][BN * BK];      // raw B tiles
+  float b_hi[STAGES][BN * BK];   // K-major hi / lo halves of B, the wgmma operands
   float b_lo[STAGES][BN * BK];
-  uint64_t full[STAGES], split[STAGES], empty[STAGES], tfull[2], tempty[2];
-  uint32_t tmem_base;
+  uint64_t full[STAGES], split[STAGES], empty[STAGES];
 };
 
-// Two-level accumulation.  The tensor core adds each k-step into the fp32 TMEM accumulator with truncation
-// (round-toward-zero), a bias of ~2^-24 |acc| per add that grows linearly with K (measured 1.3e-5 at K=1536).
-// So TMEM only ever holds a CHUNK of CH k-blocks (CH*4 k-steps); each finished chunk is drained by the
-// accumulator warps into fp32 REGISTERS with round-to-nearest FADDs while the tensor core fills the other
-// TMEM buffer.
+// Two-level accumulation.  The tensor core adds each k-step into its fp32 accumulator with truncation
+// (round-toward-zero), a bias of ~2^-24 |acc| per add that grows linearly with K.  So the wgmma accumulator only ever
+// holds a CHUNK of CH k-blocks (CH*4 k-steps); each finished chunk is added into the running fp32 sum with
+// round-to-nearest FADDs.
 constexpr int CH = 4;
 
 constexpr int MODE_GEMM = 0, MODE_DOWN = 1, MODE_UP = 2;
 // MODE_UP4: ConvTranspose2d forward with all four output parity classes in ONE 128-column tile (Cout == 32): the K loop walks
 // the 9 shifted input windows (dy, dx in {-1, 0, 1}) instead of 4 parities x 4 taps, so every input tile is fetched from L2
-// 9 times instead of 16 (the per-parity launch ran at the L2 -> SM bandwidth: 1.07 GB per call at 1024 x 16x16x64 inputs),
-// the B tile is the parity-major weight [4 * Cout][9 * Cin] with zeros where a (parity, shift) pair does not exist, and the
-// epilogue scatters column group p to output pixel (2y + py, 2x + px).
+// 9 times instead of 16, the B tile is the parity-major weight [4 * Cout][9 * Cin] with zeros where a (parity, shift) pair
+// does not exist, and the epilogue scatters column group p to output pixel (2y + py, 2x + px).
 constexpr int MODE_UP4 = 3;
 constexpr int GROUP_M = 16;
 struct TileGeo {
@@ -239,7 +201,7 @@ struct TileGeo {
   int mtiles;              // number of M tiles
   int ntiles;              // number of N tiles.  A CTA walks the flattened (m, n) tile list blockIdx.y, blockIdx.y +
                            // gridDim.y, ... (persistent); consecutive ids cover GROUP_M m-tiles x all n-tiles column by
-                           // column, so the ~148 tiles in flight share few operand panels in L2
+                           // column, so the tiles in flight share few operand panels in L2
   int wg;                  // GEMM mode, conv weight gradient: A rows = (tap, big channel), K = small-grid pixels gathered
                            // from the channel-last big image by 4-D TMA boxes of 32 pixels (Cout = big channels)
 };
@@ -248,6 +210,7 @@ template <int BN, int PASSES>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, float* __restrict__ C,
                const float* __restrict__ bias, int M, int N, int K, int ldc, int accumulate, const TileGeo geo) {
+  constexpr int STAGES = Smem<BN>::STAGES;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   Smem<BN>& s = *reinterpret_cast<Smem<BN>*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -260,14 +223,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     tm = first + (r - tn * gsz);
   };
   // split-K (GEMM mode): blockIdx.z owns k-blocks [kb_base, kb_base + nkb); its partial tile goes to the workspace and
-  // the LAST split to arrive for an output tile sums all partials in split order (bit-reproducible, no atomics on C)
+  // a reduce kernel sums all partials in split order (bit-reproducible, no atomics on C)
   int kb_base = 0, nkb = (K + BK - 1) / BK;
   if (geo.mode == MODE_GEMM && geo.ksplits > 1) {
     const int per = (nkb + geo.ksplits - 1) / geo.ksplits;
     kb_base = (int)blockIdx.z * per;
     nkb = min(per, nkb - kb_base);
   }
-  const int nchunks = (nkb + CH - 1) / CH;
   // conv modes: a tile's origin on the small-image grid; blockIdx.z = output parity class (up)
   const int py = (int)blockIdx.z >> 1, px = (int)blockIdx.z & 1;
   auto tile_origin = [&](int id, int& tx0, int& ty0, int& tn0) {
@@ -275,300 +237,228 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     ty0 = ((id / geo.tiles_x) % geo.tiles_y) * geo.bh;
     tn0 = (id / (geo.tiles_x * geo.tiles_y)) * geo.bn;
   };
-  // Tensor memory: two accumulator buffers (2*BN columns) + per stage the A operand as hi | lo (2 x 32 columns): the
-  // A halves are read by the tensor core from TMEM instead of shared memory, which removes half of the operand traffic
-  // of a shared-memory-bandwidth-bound kernel (ncu: LSU + tensor-core wavefronts = 84 % of the smem pipe).
-  constexpr uint32_t TMEM_COLS = 512;
-  constexpr uint32_t A_TMEM0 = 2 * BN;     // column of stage 0's A hi; stage st: + 64*st; lo: + 32
-  constexpr int ACC_COLS = BN / 2;         // columns per accumulator warp (two warps share a TMEM lane quarter)
-  // instruction descriptor: D=f32, A=B=tf32, both K-major, N>>3 at [17,23), M>>4 at [24,29)
-  constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&s.full[i], 1);
-      mbar_init(&s.split[i], (PASSES == 3 ? 2 : 1) * (NSPLIT_THREADS / 32));
-      mbar_init(&s.empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s.tfull[i], 1);
-      mbar_init(&s.tempty[i], NACC_WARPS);
+      mbar_init(&s.split[i], NSPLIT_THREADS / 32);
+      mbar_init(&s.empty[i], NCONS_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) tmem_alloc(&s.tmem_base, TMEM_COLS);
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = s.tmem_base;
 
-  if (warp == 0) {
-    // ===== TMA producer (warp-uniform loop, the elected lane issues: see the MMA issuer)
-    {
+  if (warp < 4) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
+    if (warp == 0) {
+      // ===== TMA producer.  The whole warp walks the loop with warp-uniform control flow; the elected lane issues.
       const bool leader = elect_one();
       int it = 0;                                  // k-blocks issued so far, across tiles: stage / phase bookkeeping
       for (int tile = blockIdx.y; tile < mtiles; tile += tstride) {
+        int tm, tn;
+        tile_mn(tile, tm, tn);
+        const int m0 = tm * BM, n0 = tn * BN;
+        int tx0 = 0, ty0 = 0, tn0 = 0;
+        if (geo.mode != MODE_GEMM) tile_origin(tm, tx0, ty0, tn0);
+        for (int kb = 0; kb < nkb; ++kb, ++it) {
+          const int st = it % STAGES;
+          if (it >= STAGES) mbar_wait(&s.empty[st], ((it / STAGES) - 1) & 1);
+          if (leader) {
+            mbar_expect_tx(&s.full[st], (uint32_t)((BM + BN) * BK * sizeof(float)));
+            if (geo.mode == MODE_GEMM) {
+              const int k0 = (kb_base + kb) * BK;
+              if (geo.wg) {
+                // k0 = first of 32 raster-consecutive small pixels (one box bw x bh x bn); block j of the tile = rows of
+                // one (tap, 32-channel chunk): the same strided gather as the forward conv, read MN-major
+                const int x0 = k0 % geo.w, y0 = (k0 / geo.w) % geo.h, i0 = k0 / (geo.w * geo.h);
+                for (int j = 0; j < BM / 32; ++j) {
+                  const int r0 = m0 + 32 * j, tap = r0 / geo.Cout, ch = r0 - tap * geo.Cout;
+                  tma_load_4d(s.a[st] + j * 1024, &mapA, &s.full[st], ch, 2 * x0 - 1 + (tap & 3), 2 * y0 - 1 + (tap >> 2), i0);
+                }
+              } else if (!geo.a_mn) tma_load_2d(s.a[st], &mapA, &s.full[st], k0, m0);
+              else
+                for (int j = 0; j < BM / 32; ++j) tma_load_2d(s.a[st] + j * 1024, &mapA, &s.full[st], m0 + 32 * j, k0);
+              if (!geo.b_mn) tma_load_2d(s.b[st], &mapB, &s.full[st], k0, n0);
+              else
+                for (int j = 0; j < BN / 32; ++j) tma_load_2d(s.b[st] + j * 1024, &mapB, &s.full[st], n0 + 32 * j, k0);
+            } else {
+              const int tap = kb / geo.chunks, ch = (kb - tap * geo.chunks) * BK;
+              int x, y;
+              if (geo.mode == MODE_DOWN)     { x = 2 * tx0 - 1 + (tap & 3); y = 2 * ty0 - 1 + (tap >> 2); }
+              else if (geo.mode == MODE_UP4) { x = tx0 + (tap % 3) - 1;     y = ty0 + (tap / 3) - 1; }      // tap = shift index
+              else                           { x = tx0 + px - (tap & 1);    y = ty0 + py - (tap >> 1); }
+              tma_load_4d(s.a[st], &mapA, &s.full[st], ch, x, y, tn0);
+              tma_load_2d(s.b[st], &mapB, &s.full[st], kb * BK, n0 + (geo.mode == MODE_UP ? (int)blockIdx.z * geo.Cout : 0));
+            }
+          }
+          __syncwarp();
+        }
+      }
+    } else {
+      // ===== B splitters: hi / lo halves of each landed B tile into the K-major swizzled operand buffers
+      const int t = threadIdx.x - 32;
+      int ntl = 0;
+      for (int tile = blockIdx.y; tile < mtiles; tile += tstride) ++ntl;
+      const int total_kb = ntl * nkb;
+      const bool b_mn = geo.b_mn != 0;
+      for (int kb = 0; kb < total_kb; ++kb) {
+        const int st = kb % STAGES;
+        mbar_wait(&s.full[st], (kb / STAGES) & 1);
+        const char* raw = reinterpret_cast<const char*>(s.b[st]);
+        char* bh = reinterpret_cast<char*>(s.b_hi[st]);
+        char* bl = reinterpret_cast<char*>(s.b_lo[st]);
+        for (int w = t; w < BN * BK / 4; w += NSPLIT_THREADS) {
+          // work item = one 16-byte chunk (row n, k = 4kc .. 4kc+3) of the K-major target.  MN-major source: a warp
+          // covers 32 consecutive n of one kc, so every gather load reads one 128-byte line (conflict-free)
+          int n, kc;
+          float4 v;
+          if (!b_mn) {
+            n = w >> 3; kc = w & 7;
+            v = *reinterpret_cast<const float4*>(raw + kmajor_off(n, 4 * kc));
+          } else {
+            n = w % BN; kc = w / BN;
+            v.x = *reinterpret_cast<const float*>(raw + mnmajor_off(n, 4 * kc));
+            v.y = *reinterpret_cast<const float*>(raw + mnmajor_off(n, 4 * kc + 1));
+            v.z = *reinterpret_cast<const float*>(raw + mnmajor_off(n, 4 * kc + 2));
+            v.w = *reinterpret_cast<const float*>(raw + mnmajor_off(n, 4 * kc + 3));
+          }
+          float4 h;
+          h.x = __uint_as_float(__float_as_uint(v.x) & 0xffffe000u);
+          h.y = __uint_as_float(__float_as_uint(v.y) & 0xffffe000u);
+          h.z = __uint_as_float(__float_as_uint(v.z) & 0xffffe000u);
+          h.w = __uint_as_float(__float_as_uint(v.w) & 0xffffe000u);
+          const uint32_t o = kmajor_off(n, 4 * kc);
+          *reinterpret_cast<float4*>(bh + o) = h;
+          if (PASSES == 3) *reinterpret_cast<float4*>(bl + o) = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy (wgmma)
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&s.split[st]);
+      }
+    }
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
+    // ===== consumers.  Warpgroup cw owns tile rows [64 cw, 64 cw + 64); warp wq of it rows 16 wq + {g, g + 8}.
+    constexpr int NACC = BN / 2;
+    const int cw = (warp >> 2) - 1, wq = warp & 3, g = lane >> 2, tq = lane & 3;
+    const int r0 = cw * 64 + wq * 16 + g;          // tile rows of this thread: r0 and r0 + 8
+    const bool a_mn_tile = geo.a_mn != 0;          // GEMM with transposed A, or the conv weight gradient
+    const uint64_t dbh_base = make_desc(smem_u32(s.b_hi[0])), dbl_base = make_desc(smem_u32(s.b_lo[0]));
+    constexpr uint64_t STAGE_STEP = (uint64_t)(BN * BK * sizeof(float)) >> 4;
+    int it = 0;
+    for (int tile = blockIdx.y; tile < mtiles; tile += tstride) {
       int tm, tn;
       tile_mn(tile, tm, tn);
       const int m0 = tm * BM, n0 = tn * BN;
       int tx0 = 0, ty0 = 0, tn0 = 0;
       if (geo.mode != MODE_GEMM) tile_origin(tm, tx0, ty0, tn0);
+      float acc[NACC], cacc[NACC];
+#pragma unroll
+      for (int j = 0; j < NACC; ++j) { acc[j] = 0.f; cacc[j] = 0.f; }
       for (int kb = 0; kb < nkb; ++kb, ++it) {
         const int st = it % STAGES;
-        if (it >= STAGES) mbar_wait(&s.empty[st], ((it / STAGES) - 1) & 1);
-        if (leader) {
-        mbar_expect_tx(&s.full[st], (uint32_t)((BM + BN) * BK * sizeof(float)));
-        if (geo.mode == MODE_GEMM) {
-          const int k0 = (kb_base + kb) * BK;
-          if (geo.wg) {
-            // k0 = first of 32 raster-consecutive small pixels (one box bw x bh x bn); block j of the tile = rows of one
-            // (tap, 32-channel chunk): the same strided gather as the forward conv, read MN-major
-            const int x0 = k0 % geo.w, y0 = (k0 / geo.w) % geo.h, i0 = k0 / (geo.w * geo.h);
-            for (int j = 0; j < BM / 32; ++j) {
-              const int r0 = m0 + 32 * j, tap = r0 / geo.Cout, ch = r0 - tap * geo.Cout;
-              tma_load_4d(s.a_hi[st] + j * 1024, &mapA, &s.full[st], ch, 2 * x0 - 1 + (tap & 3), 2 * y0 - 1 + (tap >> 2), i0);
-            }
-          } else if (!geo.a_mn) tma_load_2d(s.a_hi[st], &mapA, &s.full[st], k0, m0);
-          else
-            for (int j = 0; j < BM / 32; ++j) tma_load_2d(s.a_hi[st] + j * 1024, &mapA, &s.full[st], m0 + 32 * j, k0);
-          if (!geo.b_mn) tma_load_2d(s.b_hi[st], &mapB, &s.full[st], k0, n0);
-          else
-            for (int j = 0; j < BN / 32; ++j) tma_load_2d(s.b_hi[st] + j * 1024, &mapB, &s.full[st], n0 + 32 * j, k0);
-        } else {
-          const int tap = kb / geo.chunks, ch = (kb - tap * geo.chunks) * BK;
-          int x, y;
-          if (geo.mode == MODE_DOWN)     { x = 2 * tx0 - 1 + (tap & 3); y = 2 * ty0 - 1 + (tap >> 2); }
-          else if (geo.mode == MODE_UP4) { x = tx0 + (tap % 3) - 1;     y = ty0 + (tap / 3) - 1; }      // tap = shift index
-          else                           { x = tx0 + px - (tap & 1);    y = ty0 + py - (tap >> 1); }
-          tma_load_4d(s.a_hi[st], &mapA, &s.full[st], ch, x, y, tn0);
-          tma_load_2d(s.b_hi[st], &mapB, &s.full[st], kb * BK, n0 + (geo.mode == MODE_UP ? (int)blockIdx.z * geo.Cout : 0));
-        }
-        }
-        __syncwarp();
-      }
-      }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer.  The WHOLE warp walks the loop with warp-uniform control flow, so stage / descriptor arithmetic
-    // stays on the uniform datapath; only the tcgen05 instructions sit behind the elected lane.  (With the loop inside
-    // `if (lane == 0)` ptxas cannot prove uniformity and rebuilds every uniform operand with ELECT + R2UR.BROADCAST: 225
-    // dependent SASS instructions per k-block made this single thread the limiter of the kernel, ncu r2_gemm_tc.)
-    const bool leader = elect_one();
-    const bool b_mn = geo.b_mn != 0;
-    // A comes from tensor memory (always [row][k]): only B's major bit depends on the operand layout
-    const uint32_t idesc = IDESC | ((uint32_t)b_mn << 16);
-    const uint64_t b_step = (b_mn ? 1024 : 32) >> 4;
-    // B descriptors of stage 0; a stage advances the 14-bit start-address field (16-byte units) by the buffer size, a
-    // k-step by 32 B inside the 128-byte swizzle row (K-major) or by 1024 B = two 4-row k atoms (MN-major)
-    const uint64_t dbh_base = b_mn ? make_desc_mn(smem_u32(s.b_hi[0])) : make_desc(smem_u32(s.b_hi[0]));
-    const uint64_t dbl_base = b_mn ? make_desc_mn(smem_u32(s.b_lo[0])) : make_desc(smem_u32(s.b_lo[0]));
-    constexpr uint64_t STAGE_STEP = (uint64_t)(BN * BK * sizeof(float)) >> 4;
-    int it = 0, gc0 = 0;                         // k-blocks / TMEM chunks issued so far, across tiles
-    for (int tile = blockIdx.y; tile < mtiles; tile += tstride, gc0 += nchunks)
-    for (int kb = 0; kb < nkb; ++kb, ++it) {
-      const int st = it % STAGES;
-      const int c = gc0 + kb / CH, buf = c & 1;
-      const bool chunk_start = (kb % CH) == 0;
-      if (chunk_start && c >= 2)             // the accumulator warps must have drained this TMEM buffer
-        mbar_wait(&s.tempty[buf], ((c >> 1) - 1) & 1);
-      mbar_wait(&s.split[st], (it / STAGES) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t acc = tmem + (uint32_t)(buf * BN);
-      const uint64_t dbh0 = dbh_base + (uint64_t)st * STAGE_STEP, dbl0 = dbl_base + (uint64_t)st * STAGE_STEP;
-      const uint32_t ta_hi = tmem + A_TMEM0 + 64u * (uint32_t)st, ta_lo = ta_hi + 32u;
-      if (leader) {
+        const uint32_t ph = (it / STAGES) & 1;
+        mbar_wait(&s.full[st], ph);
+        mbar_wait(&s.split[st], ph);
+        // A fragment of the 4 k-steps (tf32 m64k8 layout: a0 (g, t), a1 (g+8, t), a2 (g, t+4), a3 (g+8, t+4))
+        const char* araw = reinterpret_cast<const char*>(s.a[st]);
+        uint32_t ahi[4][4], alo[4][4];
 #pragma unroll
-        for (int k4 = 0; k4 < BK / 8; ++k4) {
-          const uint64_t ob = (uint64_t)k4 * b_step;
+        for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int r = r0 + 8 * (e & 1), k = 8 * ks + tq + 4 * (e >> 1);
+            const uint32_t x = *reinterpret_cast<const uint32_t*>(araw + (a_mn_tile ? mnmajor_off(r, k) : kmajor_off(r, k)));
+            ahi[ks][e] = x & 0xffffe000u;
+            if (PASSES == 3) alo[ks][e] = __float_as_uint(__uint_as_float(x) - __uint_as_float(x & 0xffffe000u));
+          }
+        const bool chunk_start = (kb % CH) == 0;
+        const uint64_t dbh0 = dbh_base + (uint64_t)st * STAGE_STEP, dbl0 = dbl_base + (uint64_t)st * STAGE_STEP;
+        fence_regs(cacc);
+        fence_regs(ahi);
+        if (PASSES == 3) fence_regs(alo);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {
+          const uint64_t ob = (uint64_t)ks * 2;    // 32 B per k-step, in 16-byte units
+          const int keep = !(chunk_start && ks == 0);
           if (PASSES == 3) {
             // small cross terms first, then the leading term
-            umma_tf32_ts(acc, ta_hi + 8u * k4, dbl0 + ob, idesc, !(chunk_start && k4 == 0));
-            umma_tf32_ts(acc, ta_lo + 8u * k4, dbh0 + ob, idesc, 1);
-            umma_tf32_ts(acc, ta_hi + 8u * k4, dbh0 + ob, idesc, 1);
+            wgmma_tf32(cacc, ahi[ks], dbl0 + ob, keep);
+            wgmma_tf32(cacc, alo[ks], dbh0 + ob, 1);
+            wgmma_tf32(cacc, ahi[ks], dbh0 + ob, 1);
           } else {
-            umma_tf32_ts(acc, ta_hi + 8u * k4, dbh0 + ob, idesc, !(chunk_start && k4 == 0));
+            wgmma_tf32(cacc, ahi[ks], dbh0 + ob, keep);
           }
         }
-        umma_commit(&s.empty[st]);   // stage reusable once these MMAs have read it
-        if ((kb % CH) == CH - 1 || kb == nkb - 1) umma_commit(&s.tfull[buf]);   // chunk complete
-      }
-      __syncwarp();
-    }
-  } else if (warp >= SPLIT_WARP0 && warp < ACC_WARP0) {
-    // ===== A splitters: hi/lo decomposition of each landed A tile into tensor memory
-    const int t = threadIdx.x - SPLIT_WARP0 * 32;
-    const bool a_mn_tile = geo.a_mn != 0;          // GEMM with transposed A, or the conv weight gradient
-    int ntl = 0;
-    for (int tile = blockIdx.y; tile < mtiles; tile += tstride) ++ntl;
-    const int total_kb = ntl * nkb;
-    for (int kb = 0; kb < total_kb; ++kb) {
-      const int st = kb % STAGES;
-      mbar_wait(&s.full[st], (kb / STAGES) & 1);
-      // thread t owns tile row t = TMEM lane t (splitter warp w reads/writes lanes [32w, 32w+32)).  It gathers the
-      // row's 32 k values from the swizzled tile, stores them (the raw bits are the hi operand: the datapath truncates)
-      // and lo = x - trunc(x) into this stage's TMEM columns.
-      const char* base = reinterpret_cast<const char*>(s.a_hi[st]);
-      uint32_t hi[32], lo[32];
-      if (!a_mn_tile) {
-        // K-major tile: row t = 128 B, 16-byte chunk c stored at position c ^ (t & 7)
-        const char* row = base + t * 128;
+        wgmma_commit();
+        wgmma_wait_all();
+        fence_regs(cacc);
+        fence_regs(ahi);
+        if (PASSES == 3) fence_regs(alo);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&s.empty[st]);   // this warp is done with the stage's A and B
+        if ((kb % CH) == CH - 1 || kb == nkb - 1) {
 #pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          const float4 v = *reinterpret_cast<const float4*>(row + ((c ^ (t & 7)) << 4));
-          hi[4 * c] = __float_as_uint(v.x); hi[4 * c + 1] = __float_as_uint(v.y);
-          hi[4 * c + 2] = __float_as_uint(v.z); hi[4 * c + 3] = __float_as_uint(v.w);
+          for (int j = 0; j < NACC; ++j) acc[j] += cacc[j];
         }
-      } else {
-        // MN-major tile: block t/32 (4 KB), k-row k = 128 B, element t%32 inside it with the 32-byte chunk index
-        // XOR-ed by k % 4 (SWIZZLE_128B_BASE32B)
-        const char* blk = base + (t >> 5) * 4096 + ((t & 7) << 2);
-        const int ch = (t & 31) >> 3;
-#pragma unroll
-        for (int k = 0; k < 32; ++k)
-          hi[k] = *reinterpret_cast<const uint32_t*>(blk + k * 128 + ((ch ^ (k & 3)) << 5));
       }
-      const uint32_t ta = tmem + (((uint32_t)(t & ~31)) << 16) + A_TMEM0 + 64u * (uint32_t)st;
-      tmem_st32(ta, hi);
-      if (PASSES == 3) {
+      // ---- epilogue.  acc[4j + 2h + e] = tile (row r0 + 8h, column 8j + 2tq + e)
 #pragma unroll
-        for (int k = 0; k < 32; ++k) {
-          const float x = __uint_as_float(hi[k]);
-          lo[k] = __float_as_uint(x - __uint_as_float(hi[k] & 0xffffe000u));
+      for (int hh = 0; hh < 2; ++hh) {
+        const int r = r0 + 8 * hh;
+        const int row = m0 + r;
+        bool row_ok = row < M;
+        size_t row_off = (size_t)row * ldc;
+        int wi = 0, hi = 0, ni = 0;
+        if (geo.mode != MODE_GEMM) {
+          wi = r % geo.bw; hi = (r / geo.bw) % geo.bh; ni = r / (geo.bw * geo.bh);
+          const int n = tn0 + ni, y = ty0 + hi, x = tx0 + wi;
+          row_ok = n < geo.NB;
+          if (geo.mode == MODE_DOWN) row_off = (((size_t)n * geo.h + y) * geo.w + x) * (size_t)ldc;
+          else row_off = (((size_t)n * (2 * geo.h) + (2 * y + py)) * (2 * geo.w) + (2 * x + px)) * (size_t)ldc;
         }
-        tmem_st32(ta + 32u, lo);
-      }
-      asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");      // the A halves have landed in TMEM
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");  // TMEM stores ordered before the arrival
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s.split[st]);
-    }
-  } else if (PASSES == 3 && (warp == 2 || warp == 3 || warp >= BSPLIT_WARP_HI)) {
-    // ===== B splitters: lo = x - trunc(x) of each landed B tile to the twin buffer (same swizzled offsets, so the split
-    // is layout-agnostic); the raw tile itself is the hi operand
-    const int t = (warp >= BSPLIT_WARP_HI ? warp - BSPLIT_WARP_HI + 2 : warp - 2) * 32 + lane;
-    int ntl = 0;
-    for (int tile = blockIdx.y; tile < mtiles; tile += tstride) ++ntl;
-    const int total_kb = ntl * nkb;
-    for (int kb = 0; kb < total_kb; ++kb) {
-      const int st = kb % STAGES;
-      mbar_wait(&s.full[st], (kb / STAGES) & 1);
-      const float4* bh = reinterpret_cast<const float4*>(s.b_hi[st]);
-      float4* bl = reinterpret_cast<float4*>(s.b_lo[st]);
+        if (geo.mode == MODE_UP4) {
+          // columns [32p, 32p + 32) of the tile = the Cout = 32 channels of output pixel (2y + (p >> 1), 2x + (p & 1))
+          if (!row_ok) continue;
+          const size_t n = (size_t)(tn0 + ni);
+          const int y = ty0 + hi, x = tx0 + wi;
 #pragma unroll
-      for (int i = 0; i < BN * BK / 4 / NSPLIT_THREADS; ++i) {
-        const int idx = t + i * NSPLIT_THREADS;
-        const float4 v = bh[idx];
-        float4 l;
-        l.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xffffe000u);
-        l.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xffffe000u);
-        l.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xffffe000u);
-        l.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xffffe000u);
-        bl[idx] = l;
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> async proxy (UMMA)
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s.split[st]);
-    }
-  } else if (warp >= ACC_WARP0 && warp < ACC_WARP0 + NACC_WARPS) {
-    // ===== accumulators + epilogue.  Warp (q, half): TMEM lanes [32q, 32q+32), columns [half*BN/2, +BN/2).
-    const int q = warp & 3, half = (warp - ACC_WARP0) >> 2;
-    int gc0 = 0;
-    for (int tile = blockIdx.y; tile < mtiles; tile += tstride, gc0 += nchunks) {
-    int tm, tn;
-    tile_mn(tile, tm, tn);
-    const int m0 = tm * BM, n0 = tn * BN;
-    int tx0 = 0, ty0 = 0, tn0 = 0;
-    if (geo.mode != MODE_GEMM) tile_origin(tm, tx0, ty0, tn0);
-    float acc[ACC_COLS];
+          for (int j = 0; j < NACC / 4; ++j) {
+            const int c = 8 * j + 2 * tq, p = c >> 5, ch = c & 31;
+            float* dst = C + ((n * (2 * geo.h) + (2 * y + (p >> 1))) * (2 * geo.w) + (2 * x + (p & 1))) * (size_t)32 + ch;
+            float2 o = make_float2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]);
+            if (bias) { o.x += bias[ch]; o.y += bias[ch + 1]; }
+            *reinterpret_cast<float2*>(dst) = o;
+          }
+          continue;
+        }
+        if (geo.mode == MODE_GEMM && (geo.ksplits > 1 || geo.force_part)) {
+          // ---- deterministic split-K: this split's partial tile goes to the workspace; splitk_reduce_kernel (launched
+          // right behind this kernel) sums the partials of every output element in split order
+          float* prow = geo.part + ((size_t)blockIdx.z * geo.mpad + (size_t)row) * geo.ldw + n0;
 #pragma unroll
-    for (int j = 0; j < ACC_COLS; ++j) acc[j] = 0.f;
-    for (int cl = 0; cl < nchunks; ++cl) {
-      const int c = gc0 + cl, buf = c & 1;
-      mbar_wait(&s.tfull[buf], (c >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+          for (int j = 0; j < NACC / 4; ++j)
+            *reinterpret_cast<float2*>(prow + 8 * j + 2 * tq) = make_float2(acc[4 * j + 2 * hh], acc[4 * j + 2 * hh + 1]);
+          continue;
+        }
+        if (!row_ok) continue;
+        float* crow = C + row_off;
 #pragma unroll
-      for (int c0 = 0; c0 < ACC_COLS; c0 += 16) {   // 16 columns at a time: 96 registers per thread (576 threads)
-        uint32_t r[16];
-        tmem_ld16(tmem + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BN + half * ACC_COLS + c0), r);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) acc[c0 + j] += __uint_as_float(r[j]);
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s.tempty[buf]);
-    }
-    const int row = m0 + q * 32 + lane;
-    bool row_ok = row < M;
-    size_t row_off = (size_t)row * ldc;
-    if (geo.mode != MODE_GEMM) {
-      const int r = q * 32 + lane;
-      const int wi = r % geo.bw, hi = (r / geo.bw) % geo.bh, ni = r / (geo.bw * geo.bh);
-      const int n = tn0 + ni, y = ty0 + hi, x = tx0 + wi;
-      row_ok = n < geo.NB;
-      if (geo.mode == MODE_DOWN) row_off = (((size_t)n * geo.h + y) * geo.w + x) * (size_t)ldc;
-      else row_off = (((size_t)n * (2 * geo.h) + (2 * y + py)) * (2 * geo.w) + (2 * x + px)) * (size_t)ldc;
-    }
-    bool store = true;
-    if (geo.mode == MODE_UP4) {
-      // columns [32p, 32p + 32) of the tile = the Cout = 32 channels of output pixel (2y + (p >> 1), 2x + (p & 1))
-      if (row_ok) {
-        const int r = q * 32 + lane;
-        const int wi = r % geo.bw, hi = (r / geo.bw) % geo.bh, ni = r / (geo.bw * geo.bh);
-        const size_t n = (size_t)(tn0 + ni);
-        const int y = ty0 + hi, x = tx0 + wi;
-#pragma unroll
-        for (int jp = 0; jp < ACC_COLS / 32; ++jp) {
-          const int p = (half * ACC_COLS) / 32 + jp;
-          float* dst = C + ((n * (2 * geo.h) + (2 * y + (p >> 1))) * (2 * geo.w) + (2 * x + (p & 1))) * (size_t)32;
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            float4 o = make_float4(acc[32 * jp + j], acc[32 * jp + j + 1], acc[32 * jp + j + 2], acc[32 * jp + j + 3]);
-            if (bias) { o.x += bias[j]; o.y += bias[j + 1]; o.z += bias[j + 2]; o.w += bias[j + 3]; }
-            *reinterpret_cast<float4*>(dst + j) = o;
+        for (int j = 0; j < NACC / 4; ++j) {
+          const int cb = n0 + 8 * j + 2 * tq;
+          float v0 = acc[4 * j + 2 * hh], v1 = acc[4 * j + 2 * hh + 1];
+          if (cb + 1 < N && ((reinterpret_cast<uintptr_t>(crow + cb) & 7) == 0)) {
+            if (bias) { v0 += bias[cb]; v1 += bias[cb + 1]; }
+            if (accumulate) { const float2 q = *reinterpret_cast<const float2*>(crow + cb); v0 += q.x; v1 += q.y; }
+            *reinterpret_cast<float2*>(crow + cb) = make_float2(v0, v1);
+          } else {
+            if (cb < N) crow[cb] = v0 + (bias ? bias[cb] : 0.f) + (accumulate ? crow[cb] : 0.f);
+            if (cb + 1 < N) crow[cb + 1] = v1 + (bias ? bias[cb + 1] : 0.f) + (accumulate ? crow[cb + 1] : 0.f);
           }
         }
       }
-      store = false;
-    }
-    if (geo.mode == MODE_GEMM && (geo.ksplits > 1 || geo.force_part)) {
-      // ---- deterministic split-K: this split's partial tile goes to the workspace; splitk_reduce_kernel (launched right
-      // behind this kernel) sums the partials of every output element in split order — no atomics, bit-reproducible
-      float* prow = geo.part + ((size_t)blockIdx.z * geo.mpad + (size_t)(m0 + q * 32 + lane)) * geo.ldw + n0 + half * ACC_COLS;
-#pragma unroll
-      for (int j = 0; j < ACC_COLS; j += 4)
-        *reinterpret_cast<float4*>(prow + j) = make_float4(acc[j], acc[j + 1], acc[j + 2], acc[j + 3]);
-      store = false;
-    }
-    if (row_ok && store) {
-      const int cb = n0 + half * ACC_COLS;
-      float* crow = C + row_off + cb;
-      const bool vec = ((reinterpret_cast<uintptr_t>(crow) & 15) == 0) && (cb + ACC_COLS <= N);
-      if (vec) {
-#pragma unroll
-        for (int j = 0; j < ACC_COLS; j += 4) {
-          float4 o = make_float4(acc[j], acc[j + 1], acc[j + 2], acc[j + 3]);
-          if (bias) { o.x += bias[cb + j]; o.y += bias[cb + j + 1]; o.z += bias[cb + j + 2]; o.w += bias[cb + j + 3]; }
-          if (accumulate) { const float4 p = *reinterpret_cast<const float4*>(crow + j); o.x += p.x; o.y += p.y; o.z += p.z; o.w += p.w; }
-          *reinterpret_cast<float4*>(crow + j) = o;
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < ACC_COLS; ++j) {
-          if (cb + j < N) {
-            float o = acc[j];
-            if (bias) o += bias[cb + j];
-            if (accumulate) o += crow[j];
-            crow[j] = o;
-          }
-        }
-      }
-    }
     }   // tile loop
-  }
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    tmem_dealloc(tmem, TMEM_COLS);
   }
 }
 
@@ -606,8 +496,8 @@ EncodeTiledFn encode_tiled() {
 }
 
 // [rows][cols] fp32, row stride ld; box = [box_rows][32], 128-byte swizzle, zero fill out of bounds
-int get_map(const float* ptr, int rows, int cols, int ld, int box_rows, CUtensorMap* out, bool atom32 = false) {
-  MapKey key{ptr, rows, cols, ld, box_rows | (atom32 ? 1 << 16 : 0)};
+int get_map(const float* ptr, int rows, int cols, int ld, int box_rows, CUtensorMap* out) {
+  MapKey key{ptr, rows, cols, ld, box_rows};
   std::lock_guard<std::mutex> lk(g_maps_mu);
   auto it = g_maps.find(key);
   if (it != g_maps.end()) { *out = it->second; return B200RL_OK; }
@@ -620,7 +510,7 @@ int get_map(const float* ptr, int rows, int cols, int ld, int box_rows, CUtensor
   if (!enc) { b200rl_set_error("cuTensorMapEncodeTiled is not available from this driver"); return B200RL_ERR_CUDA; }
   CUresult r = enc(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), dims, strides, box,
                                       estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                      atom32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                                      CU_TENSOR_MAP_SWIZZLE_128B,
                                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     b200rl_set_error("cuTensorMapEncodeTiled failed (%d) for [%d x %d] ld %d", (int)r, rows, cols, ld);
@@ -650,9 +540,8 @@ struct Map4Hash {
 std::unordered_map<Map4Key, CUtensorMap, Map4Hash> g_maps4;
 
 // channel-last image [N][H][W][C]; box = {32 ch, bw px, bh px, bn images} sampled with element stride es in W and H
-int get_map4(const float* ptr, int C, int W, int H, int N, int bw, int bh, int bn, int es, CUtensorMap* out,
-             bool atom32 = false) {
-  Map4Key key{ptr, C, W, H, N, bw, bh, bn, es | (atom32 ? 1 << 8 : 0)};
+int get_map4(const float* ptr, int C, int W, int H, int N, int bw, int bh, int bn, int es, CUtensorMap* out) {
+  Map4Key key{ptr, C, W, H, N, bw, bh, bn, es};
   std::lock_guard<std::mutex> lk(g_maps_mu);
   auto it = g_maps4.find(key);
   if (it != g_maps4.end()) { *out = it->second; return B200RL_OK; }
@@ -666,7 +555,7 @@ int get_map4(const float* ptr, int C, int W, int H, int N, int bw, int bh, int b
   if (!enc) { b200rl_set_error("cuTensorMapEncodeTiled is not available from this driver"); return B200RL_ERR_CUDA; }
   CUresult r = enc(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(ptr), dims, strides, box,
                                       estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                      atom32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                                      CU_TENSOR_MAP_SWIZZLE_128B,
                                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     b200rl_set_error("cuTensorMapEncodeTiled(4D) failed (%d) for image [%d,%d,%d,%d]", (int)r, N, H, W, C);
@@ -689,9 +578,8 @@ bool conv_tile(int h, int w, int NB, int* bw, int* bh, int* bn) {
 }
 
 // Persistent scheduling: with one CTA per SM (the operand stages fill shared memory) a launch of many short tiles pays
-// TMEM allocation, barrier setup, pipeline fill and an un-overlapped epilogue per tile.  When there are more than two
-// waves of tiles, launch about one CTA per SM and let each walk its M tiles (the epilogue of a tile overlaps the main
-// loop of the next through the double-buffered TMEM accumulator).
+// barrier setup and pipeline fill per tile.  When there are more than two waves of tiles, launch about one CTA per SM
+// and let each walk its M tiles (the producer already loads the next tile's stages during the epilogue of a tile).
 static unsigned persistent_grid_y(int tiles, unsigned gz) {
   const long long total = (long long)tiles * gz;
   if (total <= 2LL * kNumSMs) return (unsigned)tiles;
@@ -923,9 +811,9 @@ int gemm_tc_impl(const float* A, const float* B, float* C, const float* bias, in
   CUtensorMap ma, mb;
   // A: [M][K] (K-major) or, transposed, [K][M] (MN-major: boxes of 32 k-rows x 32 m);  B: [N][K] or [K][N]
   if (!transA) { if (int rc = get_map(A, M, K, lda, BM, &ma)) return rc; }
-  else         { if (int rc = get_map(A, K, M, lda, 32, &ma, true)) return rc; }
+  else         { if (int rc = get_map(A, K, M, lda, 32, &ma)) return rc; }
   if (transB)  { if (int rc = get_map(B, N, K, ldb, BN, &mb)) return rc; }
-  else         { if (int rc = get_map(B, K, N, ldb, 32, &mb, true)) return rc; }
+  else         { if (int rc = get_map(B, K, N, ldb, 32, &mb)) return rc; }
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
   TileGeo g = {};
   g.mode = MODE_GEMM;
@@ -1119,8 +1007,8 @@ extern "C" int b200rl_conv_wgrad_mn(const float* small_, const float* big, float
   g.h = h; g.w = w; g.NB = NB; g.Cout = Cb;
   g.bw = w < 32 ? w : 32; g.bh = (32 / g.bw) < h ? (32 / g.bw) : h; g.bn = 32 / (g.bw * g.bh);
   CUtensorMap ma, mb;
-  if (int rc = get_map4(big, Cb, 2 * w, 2 * h, NB, g.bw, g.bh, g.bn, 2, &ma, true)) return rc;
-  if (int rc = get_map(small_, P, Cs, Cs, 32, &mb, true)) return rc;
+  if (int rc = get_map4(big, Cb, 2 * w, 2 * h, NB, g.bw, g.bh, g.bn, 2, &ma)) return rc;
+  if (int rc = get_map(small_, P, Cs, Cs, 32, &mb)) return rc;
   const int BN = (N <= 64) ? 64 : 128;
   dim3 grid((N + BN - 1) / BN, M / BM);
   const int tiles = grid.x * grid.y, nkb = P / BK;

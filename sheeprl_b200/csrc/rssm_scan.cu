@@ -35,7 +35,7 @@
 
 namespace {
 
-constexpr int SCAN_G = 128;    // CTAs (one per SM; 148 SMs available)
+constexpr int SCAN_G = 128;    // CTAs (one per SM; 132 SMs available)
 constexpr int SCAN_NT = 512;   // threads per CTA: the scan is latency-bound (ncu: 11 stall cycles per issued instruction at
                                // 8 warps / SM), so every phase is spread over 32 warps with short per-warp instruction streams
 constexpr int SCAN_NW = SCAN_NT / 32;

@@ -607,7 +607,7 @@ class DV3Engine:
         # finishes those three ranges in REVERSE order, so each is all-reduced on a side stream as soon as it is final
         # (the reference's DDP buckets, fabric.backward dreamer_v3.py:191, overlap the same way)
         b_enc, b_tail = self._wm_buckets()
-        # default: overlap unless the persistent scan kernels run — they hold 128 of the 148 SMs with all of their shared
+        # default: overlap unless the persistent scan kernels run — they hold 128 of the 132 SMs with all of their shared
         # memory, NCCL's CTAs then only fit on the other 20 and the reductions get slower than one call in front of the
         # optimizer (measured at 2 GPUs: 16.96 vs 16.73 ms / step); per-step scans (XL) leave room and overlap pays
         overlap = self.allreduce_async is not None and bool(self.cfg.algo.get("overlap_allreduce", not self.fused_scan))

@@ -2,7 +2,7 @@
 
 `CudaOps` exposes one method per entry point, taking torch tensors purely as (device pointer, shape,
 leading dimension) carriers; all work is enqueued on torch's current CUDA stream.  There is NO
-fallback: constructing `CudaOps` without the built library or without an sm_100 GPU raises.
+fallback: constructing `CudaOps` without the built library or without an sm_90 (H100) GPU raises.
 """
 from __future__ import annotations
 
@@ -30,7 +30,7 @@ def load_library(path: str = LIB_PATH) -> ctypes.CDLL:
     if _lib is None:
         if not os.path.exists(path):
             raise B200RLError(
-                f"{path} not found: build it with `python -m sheeprl_b200.build` (nvcc, sm_100a). "
+                f"{path} not found: build it with `python -m sheeprl_b200.build` (nvcc, sm_90a). "
                 "The B200 engine has no CPU / PyTorch fallback.")
         _lib = ctypes.CDLL(path)
         _lib.b200rl_last_error.restype = ctypes.c_char_p
@@ -100,7 +100,7 @@ class CudaOps:
         if self.lib.b200rl_device_check() != 0:
             raise B200RLError(self.lib.b200rl_last_error().decode())
         self.launches = 0
-        self.use_tc = os.environ.get("B200RL_DISABLE_TC", "0") != "1"   # tensor-core (tcgen05) paths
+        self.use_tc = os.environ.get("B200RL_DISABLE_TC", "0") != "1"   # tensor-core (wgmma) paths
         self._pack_bufs = {}
         self._scratch_bufs = {}
 
@@ -133,7 +133,7 @@ class CudaOps:
         assert (A.shape[1] if transA else A.shape[0]) == M, (A.shape, C.shape, transA)
         assert (B.shape[0] if transB else B.shape[1]) == N and (B.shape[1] if transB else B.shape[0]) == K, \
             (A.shape, B.shape, C.shape, transA, transB)
-        # every layout goes to one entry point: transposed operands are read in place as MN-major tcgen05 operands
+        # every layout goes to one entry point: transposed operands are read in place as MN-major tiles
         self._ck(self.lib.b200rl_gemm_f32(_p(A), _p(B), _p(C), _p(bias), c_int(M), c_int(N), c_int(K), c_int(_ld(A)),
                                           c_int(_ld(B)), c_int(_ld(C)), c_int(int(transA)), c_int(int(transB)),
                                           c_int(int(accumulate)), self._st()))

@@ -1,4 +1,4 @@
-"""End-to-end parity of the CUDA engine (every op through the C-ABI) on a B200:
+"""End-to-end parity of the CUDA engine (every op through the C-ABI) on an H100:
   * against the committed reference fixtures (tests/golden, produced by the unmodified reference train());
   * against the oracle on the BASELINE config (S, B=16, T=64, H=15), incl. gradients;
   * size-independent properties at full size (finite, deterministic replay, sample one-hotness)."""

@@ -44,10 +44,10 @@ GEMM_SHAPES = [
     (1024, 512, 1536, False, True), (1024, 1536, 255, False, False), (255, 512, 1024, True, False),
     (300, 70, 33, False, True), (7, 3, 5, False, True), (5, 1, 129, False, True), (1000, 2, 512, False, True),
     (2, 512, 1000, True, False), (130, 130, 70, True, True), (64, 4096, 200, False, True),
-    # tensor-core (tcgen05 3xTF32) eligible: NT, M >= 256, N >= 48, 16-byte aligned rows
+    # tensor-core (wgmma 3xTF32) eligible: NT, M >= 256, N >= 48, 16-byte aligned rows
     (16384, 512, 1536, False, True), (1024, 255, 512, False, True), (15360, 512, 512, False, True),
     (1000, 72, 40, False, True), (257, 129, 36, False, True), (1024, 4096, 1536, False, True),
-    # transposed operands are read in place as MN-major tcgen05 operands: input gradients (NN), weight gradients (TN)
+    # transposed operands are read in place as MN-major tiles: input gradients (NN), weight gradients (TN)
     (16384, 1536, 512, False, False), (1024, 512, 255, False, False), (512, 1536, 16384, True, False),
     (255, 512, 15360, True, False), (4096, 1536, 1024, True, False), (1024, 4608, 512, False, False),
     # MN-major operands with ragged tiles in every dimension (TMA zero fill on both box axes)
@@ -60,7 +60,7 @@ GEMM_SHAPES = [
 
 
 def test_gemm_tensor_core_path_is_taken_and_exact_enough(ops):
-    """The tcgen05 path must (a) be selected for the big NT products, (b) keep fp32-level accuracy (3xTF32)."""
+    """The tensor-core path must (a) be selected for the big NT products, (b) keep fp32-level accuracy (3xTF32)."""
     import ctypes
 
     cu, em = ops
@@ -246,7 +246,7 @@ CONV_SHAPES = [(3, 8, 8, 16, 8), (2, 4, 4, 32, 16), (5, 16, 16, 4, 3), (2, 32, 3
                (3, 32, 32, 64, 3), (2, 32, 32, 96, 3), (2, 5, 32, 32, 3), (1, 12, 32, 64, 3), (5, 1, 32, 96, 3),
                # tensor-core implicit-GEMM eligible (gathered image has a multiple of 32 channels, grid tiles by 128 px)
                (8, 4, 4, 64, 32), (2, 32, 32, 32, 64), (4, 16, 16, 128, 64), (16, 8, 8, 256, 128), (24, 4, 4, 96, 32),
-               # weight gradient with operands read in place (MN-major tcgen05): k-block = part of a row / rows / images
+               # weight gradient with operands read in place (MN-major tiles): k-block = part of a row / rows / images
                (64, 4, 4, 256, 128), (2, 32, 32, 64, 32), (1, 64, 64, 48, 32), (32, 8, 8, 128, 64)]
 
 

@@ -26,7 +26,7 @@ def test_library_exports_every_declared_symbol(built):
 def test_library_identity(built):
     lib = L.load_library()
     assert lib.b200rl_abi_version() == 1
-    assert lib.b200rl_build_arch() == b"sm_100a"
+    assert lib.b200rl_build_arch() == b"sm_90a"
 
 
 def test_product_path_refuses_to_run_without_gpu():

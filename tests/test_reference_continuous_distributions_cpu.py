@@ -15,7 +15,7 @@ from oracle import dv3_oracle as O
 from oracle import ref_harness
 from tests.helpers import load_fixture
 
-pytestmark = pytest.mark.skipif(not ref_harness.reference_available(), reason="reference tree not present")
+needs_reference = pytest.mark.skipif(not ref_harness.reference_available(), reason="reference tree not present")
 
 
 def _setup(dist_type):
@@ -26,6 +26,7 @@ def _setup(dist_type):
     return fx, cfg
 
 
+@needs_reference
 @pytest.mark.parametrize("dist_type", ["tanh_normal", "normal"])
 def test_reference_train_fails_with_this_distribution(dist_type):
     from oracle import ref_run
@@ -37,6 +38,7 @@ def test_reference_train_fails_with_this_distribution(dist_type):
         ref_run.run_reference_train(cfg, adim, data, [fx["noise"][0]], n_steps=1, state=fx["init"], is_continuous=True)
 
 
+@needs_reference
 def test_reference_train_runs_with_the_supported_distribution():
     """control: the same harness and fixture DO run with scaled_normal (what the fixture was generated with)"""
     from oracle import ref_run

@@ -1,5 +1,5 @@
-// Microbenchmark: throughput / latency of the warp-level mma.sync.m16n8k8 TF32 (HMMA.1688.F32.TF32) on sm_100a,
-// against packed fp32 FMAs, per SM sub-partition.   nvcc -gencode arch=compute_100a,code=sm_100a -O3 mma_rate.cu
+// Microbenchmark: throughput / latency of the warp-level mma.sync.m16n8k8 TF32 (HMMA.1688.F32.TF32) on sm_90a,
+// against packed fp32 FMAs, per SM sub-partition.   nvcc -gencode arch=compute_90a,code=sm_90a -O3 mma_rate.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __device__ __forceinline__ void mma(float (&d)[4], unsigned a0, unsigned a1, unsigned a2, unsigned a3, unsigned b0, unsigned b1) {
