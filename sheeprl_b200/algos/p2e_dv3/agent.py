@@ -49,7 +49,8 @@ def build_agent(
     wm_scale = {"rssm.transition_model._model.3.weight": 1.0, "rssm.representation_model._model.3.weight": 1.0,
                 f"reward_model._model.{3 * nh}.weight": 0.0, f"continue_model._model.{3 * nh}.weight": 1.0,
                 **{f"observation_model.mlp_decoder.heads.{i}.weight": 1.0 for i in range(len(mlp_keys))}} if haf else {}
-    ac_scale = {f"mlp_heads.{i}.weight": 1.0 for i in range(len(actions_dim))} if haf else {}
+    n_heads = 1 if is_continuous else len(actions_dim)
+    ac_scale = {f"mlp_heads.{i}.weight": 1.0 for i in range(n_heads)} if haf else {}
     cr_scale = {f"_model.{3 * nh}.weight": 0.0} if haf else {}
     eng.wm.load(initial_state(eng.wm, wm_scale, g) if world_model_state is None else world_model_state)
     eng.actor.load(initial_state(eng.actor, ac_scale, g) if actor_task_state is None else actor_task_state)

@@ -1,6 +1,7 @@
 """Kernel schedule of one Plan2Explore (Dreamer-V3) exploration update — SURVEY §8f-4.
 
-Reference being replaced: `train` sheeprl/algos/p2e_dv3/p2e_dv3_exploration.py:41-520 (discrete actions).  The world
+Reference being replaced: `train` sheeprl/algos/p2e_dv3/p2e_dv3_exploration.py:41-520 (discrete or continuous
+`scaled_normal` actions).  The world
 model, the rollout machinery, the actor / critic updates and every kernel are the Dreamer-V3 engine's
 (`sheeprl_b200/engine.py`); this class adds what Plan2Explore adds:
 
@@ -11,7 +12,10 @@ model, the rollout machinery, the actor / critic updates and every kernel are th
     values, its reward (intrinsic = variance of the ensemble's next-state predictions, mean over the state, times
     `intrinsic_reward_multiplier`; or the task reward head), its lambda-values and Moments; the advantages are mixed
     by weight — the policy loss is linear in the advantage, so the fused policy kernel runs once per critic with
-    scale = weight share and the entropy bonus folded into the first call;
+    scale = weight share and the entropy bonus folded into the first call.  Continuous actions (objective = advantage,
+    :314-315): each critic's lambda-values and baseline (and the reward head, for task-reward critics) send their
+    weight share of the gradient into the imagined states, and ONE backward through the rollout carries the sum into
+    the exploration actor; the ensembles see the detached trajectory (:279-283), so the intrinsic reward is a constant;
   * the task behaviour (:397-474): the plain Dreamer-V3 behaviour step on the task actor / critic.
 """
 from __future__ import annotations
@@ -47,15 +51,13 @@ class P2EDV3Engine(DV3Engine):
 
     def __init__(self, cfg, actions_dim: Sequence[int], in_channels: int = 3, device="cuda", ops=None,
                  is_continuous: bool = False, mlp_dims=None):
-        if is_continuous:
-            raise NotImplementedError("Plan2Explore on the B200 engine: discrete actions only (continuous actions need the "
-                                      "intrinsic reward's gradient through the ensembles)")
-        super().__init__(cfg, actions_dim, in_channels, device, ops, is_continuous=False, mlp_dims=mlp_dims)
+        super().__init__(cfg, actions_dim, in_channels, device, ops, is_continuous=is_continuous, mlp_dims=mlp_dims)
         a = cfg.algo
         N, H, L, A, Z = self.N, self.H, self.L, self.A, self.Z
         M1, M0 = (H + 1) * N, H * N
         b = self._buf
-        _, ac_s, cr_s, _ = dv3_param_shapes(cfg, self.actions_dim, in_channels, False, dict(zip(self.vec_keys, self.vec_dims)))
+        _, ac_s, cr_s, _ = dv3_param_shapes(cfg, self.actions_dim, in_channels, self.is_continuous,
+                                            dict(zip(self.vec_keys, self.vec_dims)))
         # ---- exploration actor and critics
         self.actor_expl = FlatGroup(ac_s, device)
         self.actor_expl_mlp = _MLP(self, self.actor_expl, "model._model.", L, self.du, self.nh, None, M1, self.eps,
@@ -70,7 +72,8 @@ class P2EDV3Engine(DV3Engine):
                     target_mlp=_MLP(self, tgt, "_model.", L, self.du, self.nh, self.bins_c, M0, self.eps, f"target_expl_{k}", False),
                     moments_state=b(f"moments_state_{k}", 2), moments_out=b(f"moments_out_{k}", 2),
                     values=b(f"values_{k}", H + 1, N), lam=b(f"lam_{k}", H, N), reward_mean=b(f"reward_mean_{k}", 1),
-                    values_mean=b(f"values_mean_{k}", 1), lam_mean=b(f"lam_mean_{k}", 1), value_loss=b(f"value_loss_{k}", 1))
+                    values_mean=b(f"values_mean_{k}", 1), lam_mean=b(f"lam_mean_{k}", 1), value_loss=b(f"value_loss_{k}", 1),
+                    policy_rows=b(f"policy_rows_{k}", M0) if self.is_continuous else None)
         if not any(c["reward_type"] == "intrinsic" for c in self.critics_expl.values()):
             raise RuntimeError("You must specify at least one intrinsic critic (`reward_type='intrinsic'`)")
         # ---- ensembles
@@ -142,21 +145,24 @@ class P2EDV3Engine(DV3Engine):
         if noise is None:
             self._draw_noise(None)                                                   # post / task rollout streams 0-2
             ops.fill_exponential(self.noise_img_state_expl.view(-1), self.rng_seed, 3, self.rng_t)
-            ops.fill_exponential(self.noise_img_action_expl.view(-1), self.rng_seed, 4, self.rng_t)
+            fill = ops.fill_normal if self.is_continuous else ops.fill_exponential
+            fill(self.noise_img_action_expl.view(-1), self.rng_seed, 4, self.rng_t)
         else:
             self._draw_noise({"post": noise["post"], "img_state": noise["img_state_task"], "img_action": noise["img_action_task"]})
             self.noise_img_state_expl.copy_(noise["img_state_expl"].reshape(H, N, Z))
             self.noise_img_action_expl.copy_(torch.cat([x for x in noise["img_action_expl"]], -1))
         self._world_model_phase(data, heads_detached=True)
         self._ensemble_learning(data)
-        # exploration rollout reads its own noise; the task rollout afterwards the base buffers
+        # the exploration rollout and its losses (the continuous backward re-reads the action noise) use their own noise;
+        # the task rollout afterwards the base buffers.  The exploration losses finish before the task rollout
+        # overwrites the kept rollout activations.
         task_noise = (self.noise_img_state, self.noise_img_action)
         self.noise_img_state, self.noise_img_action = self.noise_img_state_expl, self.noise_img_action_expl
         try:
             self._imagine(self.actor_expl, self.actor_expl_mlp)
+            self._exploration_losses()
         finally:
             self.noise_img_state, self.noise_img_action = task_noise
-        self._exploration_losses()
         self._imagine()
         self._behaviour_losses()
         return self.metrics
@@ -213,7 +219,7 @@ class P2EDV3Engine(DV3Engine):
         c_logit = self.cont_img.forward(traj2)
         mo = a.actor.moments
         weights_sum = sum(c["weight"] for c in self.critics_expl.values())
-        v_logits = {}
+        v_logits, r_logits = {}, None
         for k, c in self.critics_expl.items():
             v_logits[k] = c["mlp"].forward(traj2)
             ops.twohot_mean(v_logits[k], TWOHOT_LOW, TWOHOT_HIGH, c["values"].view(-1))
@@ -232,18 +238,29 @@ class P2EDV3Engine(DV3Engine):
                                float(mo.percentile.low), float(mo.percentile.high), c["moments_out"])
             ops.sum_rows(c["values"].view(M1, 1), c["values_mean"], 1.0 / M1)
             ops.sum_rows(c["lam"].view(M0, 1), c["lam_mean"], 1.0 / M0)
-        # ---- policy: loss = -mean(D * (logp * sum_k share_k * adv_k + ent_coef * ent)); linear in the advantage
         ops.zero(self.p2e_metrics[1:2])
-        for j, (k, c) in enumerate(self.critics_expl.items()):
-            share = c["weight"] / weights_sum
-            rows, draw = (self.policy_rows, self.d_actor_raw) if j == 0 else (self.policy_rows_k, self.d_actor_raw_k)
-            ops.actor_loss_grad(self.actor_raw[:M0], self.actions.view(M1, self.A)[:M0], c["lam"].view(-1),
-                                c["values"].view(-1)[:M0], self.discount.view(-1)[:M0], c["moments_out"], self.actions_dim,
-                                self.unimix, float(a.actor.ent_coef) / share if j == 0 else 0.0, share / M0, rows, draw)
-            ops.sum_rows(rows.view(M0, 1), self.p2e_metrics[2:3], -share / M0)
-            ops.axpy(self.p2e_metrics[2:3], self.p2e_metrics[1:2])
-            if j > 0:
-                ops.axpy(self.d_actor_raw_k, self.d_actor_raw)
+        if self.is_continuous:
+            # ---- policy: loss = -mean(D * (sum_k share_k * adv_k + ent_coef * ent)), differentiated through the rollout
+            self._continuous_policy_gradient(c_logit, [
+                (c["mlp"], v_logits[k], c["values"], c["lam"], c["moments_out"], c["weight"] / weights_sum,
+                 None if c["reward_type"] == "intrinsic" else r_logits, c["policy_rows"])
+                for k, c in self.critics_expl.items()])
+            for c in self.critics_expl.values():
+                ops.sum_rows(c["policy_rows"].view(M0, 1), self.p2e_metrics[2:3], -c["weight"] / weights_sum / M0)
+                ops.axpy(self.p2e_metrics[2:3], self.p2e_metrics[1:2])
+        else:
+            # ---- policy: loss = -mean(D * (logp * sum_k share_k * adv_k + ent_coef * ent)); linear in the advantage
+            for j, (k, c) in enumerate(self.critics_expl.items()):
+                share = c["weight"] / weights_sum
+                rows, draw = (self.policy_rows, self.d_actor_raw) if j == 0 else (self.policy_rows_k, self.d_actor_raw_k)
+                ops.actor_loss_grad(self.actor_raw[:M0], self.actions.view(M1, self.A)[:M0], c["lam"].view(-1),
+                                    c["values"].view(-1)[:M0], self.discount.view(-1)[:M0], c["moments_out"],
+                                    self.actions_dim, self.unimix, float(a.actor.ent_coef) / share if j == 0 else 0.0,
+                                    share / M0, rows, draw)
+                ops.sum_rows(rows.view(M0, 1), self.p2e_metrics[2:3], -share / M0)
+                ops.axpy(self.p2e_metrics[2:3], self.p2e_metrics[1:2])
+                if j > 0:
+                    ops.axpy(self.d_actor_raw_k, self.d_actor_raw)
         self._actor_update(self.actor_expl, self.actor_expl_mlp, "actor_expl", 4)
         for j, (k, c) in enumerate(self.critics_expl.items()):
             self._critic_update(c["group"], c["mlp"], c["target_mlp"], v_logits[k], c["lam"], c["value_loss"],

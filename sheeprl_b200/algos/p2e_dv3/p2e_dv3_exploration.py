@@ -48,8 +48,8 @@ def train(
     eng = getattr(world_model, "_b200_engine", None)
     if eng is None or not hasattr(eng, "critics_expl"):
         raise TypeError("train() needs the modules returned by sheeprl_b200.algos.p2e_dv3.agent.build_agent")
-    if is_continuous:
-        raise NotImplementedError("Plan2Explore on the B200 engine: discrete actions only")
+    if bool(is_continuous) != eng.is_continuous:
+        raise ValueError("is_continuous differs from the value build_agent() was called with")
     bind = lambda m, st: m is not None and m.low.data_ptr() != st.data_ptr() and m.bind(st)  # noqa: E731
     bind(moments_task, eng.moments_state)
     for k, c in eng.critics_expl.items():

@@ -22,6 +22,8 @@ def train(fabric, world_model, actor, critic, target_critic, world_optimizer, ac
     eng = getattr(world_model, "_b200_engine", None)
     if not isinstance(eng, DV3Engine):
         raise TypeError("train() needs the modules returned by sheeprl_b200.algos.p2e_dv3.agent.build_agent")
+    if bool(is_continuous) != eng.is_continuous:
+        raise ValueError("is_continuous differs from the value build_agent() was called with")
     if moments is not None and getattr(moments, "low", None) is not None and moments.low.data_ptr() != eng.moments_state.data_ptr():
         moments.bind(eng.moments_state)
     DV3Engine.train_step(eng, data, noise)

@@ -1135,26 +1135,34 @@ class DV3Engine:
                 off += ad
 
 
-    def _continuous_policy_gradient(self, v_logits, r_logits, c_logit):
+    def _continuous_policy_gradient(self, c_logit, critics):
         """Continuous actions: objective = advantage (dreamer_v3.py:283-284), so d(policy_loss) flows from the
         lambda-values and the baseline through the critic / reward heads into the imagined states, back through the
         15 dynamics steps (straight-through prior samples, transition MLP, GRU, Linear([z, a])) into each step's
         action and from there into the actor head.  World-model / critic weights are constants here (the reference
-        discards their gradients from this loss): every product is a data-gradient product."""
+        discards their gradients from this loss): every product is a data-gradient product.
+        critics: one (mlp, v_logits, values, lam, moments_out, share, r_logits, rows) per critic whose advantage enters
+        the objective with weight `share` (Dreamer-V3: the task critic alone, share 1; Plan2Explore: every exploration
+        critic).  r_logits: the reward head's logits when that critic's reward is the task reward, None when it is a
+        constant of the loss (the intrinsic reward).  rows[m] = discount * (advantage + entropy bonus / share); the
+        bonus is counted in the first critic's rows only, its gradient once in the rollout backward."""
         ops, N, H, Z, R, L, A = self.ops, self.N, self.H, self.Z, self.R, self.L, self.A
         a = self.cfg.algo
         ac = a.actor
         M1, M0 = (H + 1) * N, H * N
         p = "rssm.recurrent_model."
         pt = "rssm.transition_model._model."
-        ops.lambda_returns_bwd(c_logit.view(H + 1, N), self.discount, self.moments_out, self.lam, self.values,
-                               self.act_ent, float(a.gamma), float(a.lmbda), float(ac.ent_coef), 1.0 / M0,
-                               self.d_values, self.d_rew, self.policy_rows.view(H, N))
-        ops.twohot_mean_bwd(v_logits, self.d_values.view(-1), TWOHOT_LOW, TWOHOT_HIGH, self.d_v_logits)
-        ops.twohot_mean_bwd(r_logits, self.d_rew.view(-1), TWOHOT_LOW, TWOHOT_HIGH, self.d_r_logits)
         traj2, d_traj2 = self.traj.view(M1, L), self.d_traj.view(M1, L)
-        self.critic_mlp.backward(traj2, self.d_v_logits, d_traj2, False, data_only=True)
-        self.rew_img.backward(traj2, self.d_r_logits, d_traj2, True, data_only=True)
+        for j, (mlp, v_logits, values, lam, moments, share, r_logits, rows) in enumerate(critics):
+            ops.lambda_returns_bwd(c_logit.view(H + 1, N), self.discount, moments, lam, values, self.act_ent,
+                                   float(a.gamma), float(a.lmbda), float(ac.ent_coef) / share if j == 0 else 0.0,
+                                   share / M0, self.d_values, self.d_rew, rows.view(H, N))
+            ops.twohot_mean_bwd(v_logits, self.d_values.view(-1), TWOHOT_LOW, TWOHOT_HIGH, self.d_v_logits)
+            if r_logits is not None:
+                ops.twohot_mean_bwd(r_logits, self.d_rew.view(-1), TWOHOT_LOW, TWOHOT_HIGH, self.d_r_logits)
+            mlp.backward(traj2, self.d_v_logits, d_traj2, j > 0, data_only=True)
+            if r_logits is not None:
+                self.rew_img.backward(traj2, self.d_r_logits, d_traj2, True, data_only=True)
         Win, Wg = self._w(p + "mlp._model.0.weight"), self._w(p + "rnn.linear.weight")
         args = (float(ac.min_std), float(ac.max_std), float(ac.init_std), float(ac.action_clip))
         ops.zero(self.cd_dz_carry)
@@ -1207,7 +1215,8 @@ class DV3Engine:
                            float(mo.percentile.low), float(mo.percentile.high), self.moments_out)
         # ---- actor (dreamer_v3.py:272-304)
         if self.is_continuous:
-            self._continuous_policy_gradient(v_logits, r_logits, c_logit)        # fills d_actor_raw, policy_rows
+            self._continuous_policy_gradient(c_logit, [(self.critic_mlp, v_logits, self.values, self.lam, self.moments_out,
+                                                        1.0, r_logits, self.policy_rows)])   # fills d_actor_raw, policy_rows
         else:
             ops.actor_loss_grad(self.actor_raw[:M0], self.actions.view(M1, self.A)[:M0], self.lam.view(-1),
                                 self.values.view(-1)[:M0], self.discount.view(-1)[:M0], self.moments_out,
