@@ -287,6 +287,28 @@ int b200rl_ppo_loss(const float* head, const float* actions, const float* old_lo
                     float* losses, int B, const int* head_dims, int n_heads, int is_continuous, int clip_vloss,
                     int normalize_adv, float clip_coef, float vf_coef, float ent_coef, cudaStream_t stream);
 
+/* The same objective over the rows whose mask[b] != 0 (recurrent PPO, ppo_recurrent.py:77-101): means over their
+ * count n (computed on the device), advantages normalised over them only when n > 1, zero dhead / dvalues on the other
+ * rows.  n == 0 gives zero losses and gradients. */
+int b200rl_ppo_loss_masked(const float* head, const float* actions, const float* old_logp, const float* adv,
+                           const float* values, const float* old_values, const float* returns, const float* mask,
+                           float* dhead, float* dvalues, float* losses, int B, const int* head_dims, int n_heads,
+                           int is_continuous, int clip_vloss, int normalize_adv, float clip_coef, float vf_coef,
+                           float ent_coef, cudaStream_t stream);
+/* Single-layer LSTM over padded time-major sequences in one launch (recurrent PPO, ppo_recurrent/agent.py:67-80; torch
+ * gate order i, f, g, o).  xw [T, B, 4H] = x W_ih^T + b_ih + b_hh; W_hh [4H, H]; h0, c0 [B, H]; lengths [B] int32 in
+ * [1, T] (sequence b is valid for t < lengths[b]).  out [T, B, H] (0 at padded steps); gates [T, B, 4H] (activated)
+ * and cs [T, B, H] (cell state) are kept for the backward, both or neither (NULL when acting); hT, cT [B, H]
+ * (nullable): the state after each sequence's last valid step. */
+int b200rl_lstm_seq_fwd(const float* xw, const float* W_hh, const float* h0, const float* c0, const int* lengths,
+                        float* out, float* gates, float* cs, float* hT, float* cT, int T, int B, int H,
+                        cudaStream_t stream);
+/* Backward through time in one launch: d_gates [T, B, 4H] = gradient w.r.t. the pre-activation gates from d_out
+ * [T, B, H] and what the forward kept; zero at padded steps.  h0 / c0 get no gradient.  The weight, bias and input
+ * gradients are dense products of d_gates done by the caller. */
+int b200rl_lstm_seq_bwd(const float* d_out, const float* W_hh, const float* gates, const float* cs, const float* c0,
+                        const int* lengths, float* d_gates, int T, int B, int H, cudaStream_t stream);
+
 /* Linear([z, a]) for a one-hot z (S groups of K classes, straight-through categorical sample) as a gather-sum over the
  * transposed weight WT [S*K + A, N]: RecurrentModel.mlp's first Linear (agent.py:328-341) inside the imagination
  * rollout.  z: [M, S*K] (row stride ldz), act: [M, A], out: [M, N]. */

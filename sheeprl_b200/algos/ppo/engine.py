@@ -340,6 +340,14 @@ class PPOEngine:
                 o.bgemm(dpre0, l0.W[:, :, :F_], b["dfeat"][:, :, :F_], aux=feat[:, :, :F_], epi="drelu", accumulate=j > 0)
             if self.Mf:
                 o.bgemm(dpre0, l0.W[:, :, F_:], b["dfeat"][:, :, F_:], accumulate=j > 0)
+        self._encoder_bwd(b, x_state)
+        self._optimizer_step()
+
+    def _encoder_bwd(self, b: dict, x_state):
+        """weight gradients of the vector and image encoders from b["dfeat"] (its image columns already masked by the
+        fc ReLU)"""
+        o, F_ = self.ops, self.F
+        B = b["dfeat"].shape[1]
         if self.menc is not None:
             dpre0, l0 = self._mlp_bwd(self.menc, b, b["dfeat"][:, :, F_:]), self.menc.lins[0]
             o.bgemm(dpre0.transpose(1, 2), x_state, l0.gW, rsum=l0.gb)
@@ -354,6 +362,9 @@ class PPOEngine:
                     o.col2im(b["dcol"][i][0], b["y"][i - 1][0].view(B, H, W, C), b["dy"][i - 1][0].view(B, H, W, C), k, st)
                 else:
                     self._bwd(self.convs[0], b["dy"][0], b["col"][0])
+
+    def _optimizer_step(self):
+        o, hp = self.ops, self.hp
         # ---- all-reduce, clip, Adam (ppo.py:92-96)
         g = self.group
         if self.allreduce is not None:

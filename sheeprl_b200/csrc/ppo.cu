@@ -76,25 +76,38 @@ struct PpoLossArgs {
   const float* actions;     // discrete: one-hot [B, sumA]; continuous: [B, A]
   const float* old_logp; const float* adv; const float* values; const float* old_values; const float* returns;
   float* dhead; float* dvalues; float* losses;   // losses[3] = policy, value, entropy
+  const float* mask;        // ppo_loss_masked only: rows with mask != 0 enter the objective
   int B, n_heads; int head_dims[8];
   int is_continuous, clip_vloss, normalize_adv;   // is_continuous: 0 discrete, 1 Normal, 2 tanh-squashed Normal
   float clip_coef, vf_coef, ent_coef;
 };
 
-// One CTA: B is a minibatch (<= a few thousand rows).
+// One CTA: B is a minibatch (<= a few thousand rows).  MASKED (ppo_recurrent.py:77-101): only rows with
+// mask != 0 count; the means are over their number n, advantages are normalised over them when n > 1, and the other
+// rows get zero gradients.
+template <bool MASKED>
 __global__ void __launch_bounds__(256) ppo_loss_kernel(const PpoLossArgs a) {
   __shared__ float red[32];
   const int B = a.B;
-  const float invB = 1.f / (float)B;
+  float n_rows = (float)B;
+  if (MASKED) {
+    float n = 0.f;
+    for (int b = threadIdx.x; b < B; b += blockDim.x) n += (a.mask[b] != 0.f) ? 1.f : 0.f;
+    n_rows = block_sum(n, red);
+  }
+  const float invB = MASKED ? (n_rows > 0.f ? 1.f / n_rows : 0.f) : 1.f / (float)B;
+  const bool normalize = a.normalize_adv && (!MASKED || n_rows > 1.f);
   // ---- advantage normalisation (utils/utils.py:121-130): (x - mean) / (std_unbiased + 1e-8)
   float mean = 0.f, inv_std = 1.f;
-  if (a.normalize_adv) {
+  if (normalize) {
     float s = 0.f;
-    for (int b = threadIdx.x; b < B; b += blockDim.x) s += a.adv[b];
+    for (int b = threadIdx.x; b < B; b += blockDim.x)
+      if (!MASKED || a.mask[b] != 0.f) s += a.adv[b];
     mean = block_sum(s, red) * invB;
     float v = 0.f;
-    for (int b = threadIdx.x; b < B; b += blockDim.x) { const float d = a.adv[b] - mean; v += d * d; }
-    v = block_sum(v, red) / (float)(B - 1);
+    for (int b = threadIdx.x; b < B; b += blockDim.x)
+      if (!MASKED || a.mask[b] != 0.f) { const float d = a.adv[b] - mean; v += d * d; }
+    v = block_sum(v, red) / (n_rows - 1.f);
     inv_std = 1.f / (sqrtf(v) + 1e-8f);
   }
   int width = 0;
@@ -104,6 +117,11 @@ __global__ void __launch_bounds__(256) ppo_loss_kernel(const PpoLossArgs a) {
   for (int b = threadIdx.x; b < B; b += blockDim.x) {
     const float* hd = a.head + (long long)b * width;
     float* dh = a.dhead + (long long)b * width;
+    if (MASKED && a.mask[b] == 0.f) {
+      for (int j = 0; j < width; ++j) dh[j] = 0.f;
+      a.dvalues[b] = 0.f;
+      continue;
+    }
     float lp = 0.f, ent = 0.f;
     // ---- pass 1: log-prob of the taken action and entropy (ppo/agent.py:179-239)
     if (a.is_continuous) {
@@ -306,7 +324,29 @@ extern "C" int b200rl_ppo_loss(const float* head, const float* actions, const fl
   for (int i = 0; i < n_heads; ++i) a.head_dims[i] = head_dims[i];
   a.is_continuous = is_continuous; a.clip_vloss = clip_vloss; a.normalize_adv = normalize_adv;
   a.clip_coef = clip_coef; a.vf_coef = vf_coef; a.ent_coef = ent_coef;
-  ppo_loss_kernel<<<1, 256, 0, st>>>(a);
+  ppo_loss_kernel<false><<<1, 256, 0, st>>>(a);
+  RL_CHECK_LAUNCH();
+  return B200RL_OK;
+}
+
+extern "C" int b200rl_ppo_loss_masked(const float* head, const float* actions, const float* old_logp, const float* adv,
+                                      const float* values, const float* old_values, const float* returns,
+                                      const float* mask, float* dhead, float* dvalues, float* losses, int B,
+                                      const int* head_dims, int n_heads, int is_continuous, int clip_vloss,
+                                      int normalize_adv, float clip_coef, float vf_coef, float ent_coef,
+                                      cudaStream_t st) {
+  RL_CHECK_ARG(head && actions && old_logp && adv && values && old_values && returns && mask && dhead && dvalues &&
+               losses, "null pointer");
+  RL_CHECK_ARG(B > 0 && n_heads > 0 && n_heads <= 8 && head_dims, "bad dims (at most 8 action heads)");
+  RL_CHECK_ARG(is_continuous >= 0 && is_continuous <= 2, "is_continuous: 0 discrete, 1 normal, 2 tanh_normal");
+  PpoLossArgs a{};
+  a.head = head; a.actions = actions; a.old_logp = old_logp; a.adv = adv; a.values = values;
+  a.old_values = old_values; a.returns = returns; a.dhead = dhead; a.dvalues = dvalues; a.losses = losses;
+  a.mask = mask; a.B = B; a.n_heads = n_heads;
+  for (int i = 0; i < n_heads; ++i) a.head_dims[i] = head_dims[i];
+  a.is_continuous = is_continuous; a.clip_vloss = clip_vloss; a.normalize_adv = normalize_adv;
+  a.clip_coef = clip_coef; a.vf_coef = vf_coef; a.ent_coef = ent_coef;
+  ppo_loss_kernel<true><<<1, 256, 0, st>>>(a);
   RL_CHECK_LAUNCH();
   return B200RL_OK;
 }

@@ -636,6 +636,43 @@ class CudaOps:
                                           c_int(int(normalize_adv)), c_float(clip_coef), c_float(vf_coef),
                                           c_float(ent_coef), self._st()))
 
+    def ppo_loss_masked(self, head, actions, old_logp, adv, values, old_values, returns, mask, dhead, dvalues, losses,
+                        head_dims, is_continuous: bool, clip_vloss: bool, normalize_adv: bool, clip_coef: float,
+                        vf_coef: float, ent_coef: float):
+        _f32(head, actions, old_logp, adv, values, old_values, returns, mask, dhead, dvalues, losses)
+        for t in (head, actions, dhead, mask):
+            assert t.is_contiguous()
+        dims = (c_int * len(head_dims))(*head_dims)
+        self._ck(self.lib.b200rl_ppo_loss_masked(_p(head), _p(actions), _p(old_logp), _p(adv), _p(values),
+                                                 _p(old_values), _p(returns), _p(mask), _p(dhead), _p(dvalues),
+                                                 _p(losses), c_int(head.shape[0]), dims, c_int(len(head_dims)),
+                                                 c_int(int(is_continuous)), c_int(int(clip_vloss)),
+                                                 c_int(int(normalize_adv)), c_float(clip_coef), c_float(vf_coef),
+                                                 c_float(ent_coef), self._st()))
+
+    # ------------------------------------------------------------------ recurrent PPO: LSTM sequences (csrc/lstm.cu)
+    def lstm_seq_fwd(self, xw, W_hh, h0, c0, lengths, out, gates=None, cs=None, hT=None, cT=None):
+        """xw [T,B,4H], W_hh [4H,H], h0/c0 [B,H], lengths int32 [B]; out [T,B,H]; gates/cs kept for the backward"""
+        _f32(xw, W_hh, h0, c0, out, gates, cs, hT, cT)
+        T, B, G = xw.shape
+        H = G // 4
+        assert lengths.dtype == torch.int32 and lengths.is_cuda and lengths.numel() == B
+        for t in (xw, W_hh, h0, c0, lengths, out, gates, cs, hT, cT):
+            assert t is None or t.is_contiguous()
+        assert W_hh.shape == (G, H) and out.numel() == T * B * H and h0.numel() == B * H and c0.numel() == B * H
+        self._ck(self.lib.b200rl_lstm_seq_fwd(_p(xw), _p(W_hh), _p(h0), _p(c0), _p(lengths), _p(out), _p(gates), _p(cs),
+                                              _p(hT), _p(cT), c_int(T), c_int(B), c_int(H), self._st()))
+
+    def lstm_seq_bwd(self, d_out, W_hh, gates, cs, c0, lengths, d_gates):
+        _f32(d_out, W_hh, gates, cs, c0, d_gates)
+        T, B, G = d_gates.shape
+        H = G // 4
+        assert lengths.dtype == torch.int32 and lengths.is_cuda and lengths.numel() == B
+        for t in (d_out, W_hh, gates, cs, c0, lengths, d_gates):
+            assert t.is_contiguous()
+        self._ck(self.lib.b200rl_lstm_seq_bwd(_p(d_out), _p(W_hh), _p(gates), _p(cs), _p(c0), _p(lengths), _p(d_gates),
+                                              c_int(T), c_int(B), c_int(H), self._st()))
+
     # ------------------------------------------------------------------ imagination: Linear([one-hot z, a]) as a gather
     def transpose2d(self, X, Y):
         """Y [cols, rows] = X [rows, cols]^T (2-D views with unit inner stride)"""
