@@ -138,8 +138,12 @@ int b200rl_kl_loss_grad(const float* post_mix, const float* prior_mix, float* d_
  * barriers (rssm_scan.cu).  The prior (transition model on the finished h sequence, agent.py:433) is NOT computed here:
  * it is off the recurrence and runs as batched products over all T*B rows (tr_pre / tr_act / prior_raw / prior_mix
  * below are unused by the kernels; the fields stay so that the per-step path and this one fill the same set of saved
- * activations).  Requires B <= 16, classes <= 32, even layer widths and the per-CTA weight slices to fit in 227 KB
- * (returns non-zero otherwise; the caller then uses the per-step ops). */
+ * activations).  Requires B <= 16, S <= 64 categoricals of D <= 32 classes, even widths (R, Dx, Dr and S*D),
+ * Dx <= 1024, R <= 1024 (at most two 4-column groups per CTA), Dr <= 4096 and the per-CTA weight slices to fit in
+ * 227 KB of shared memory; the backward kernel needs more of it than the forward, so b200rl_rssm_scan_bwd_check can
+ * refuse a model the forward runs.  Returns non-zero otherwise; the caller then uses the per-step ops.
+ * Checked against a float64 reference (tests/test_gpu_rssm_scan.py) at widths up to R = Dx = 520 and Dx = 1024, one to
+ * sixteen rows, S = 1 .. 64 and D = 1 .. 32. */
 typedef struct b200rl_rssm_scan_args {
   int T, B, S, D, R, A, Dx, Dt, Dr, ld_lat, ld_wr1;
   float eps, unimix;

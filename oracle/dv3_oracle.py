@@ -205,15 +205,18 @@ def decoder_forward(wm: Dict[str, Tensor], latent: Tensor, stages: int, eps: flo
     return x.reshape(*lead, *out_shape)
 
 
-def recurrent_step(wm: Dict[str, Tensor], z: Tensor, a: Tensor, h: Tensor, eps: float) -> Tensor:
+def recurrent_step(wm: Dict[str, Tensor], z: Tensor, a: Tensor, h: Tensor, eps: float,
+                   saves: Optional[Dict[str, Tensor]] = None) -> Tensor:
     """RecurrentModel.forward (agent.py:328-341) + LayerNormGRUCell (models.py:370-410):
     x = SiLU(LN(W_in [z,a])); g = LN(W_g [h,x]); r,c,u = chunk(g); h' = u'*tanh(sig(r)*c) + (1-u')*h,
-    u' = sig(u - 1)."""
+    u' = sig(u - 1).  `saves`: if given, receives the intermediates x_pre, x_act, g_pre, g_ln (graph nodes)."""
     p = "rssm.recurrent_model."
-    x = F.linear(torch.cat((z, a), -1), wm[p + "mlp._model.0.weight"])
-    x = F.silu(layer_norm(x, wm[p + "mlp._model.1.weight"], wm[p + "mlp._model.1.bias"], eps))
-    g = F.linear(torch.cat((h, x), -1), wm[p + "rnn.linear.weight"])
-    g = layer_norm(g, wm[p + "rnn.layer_norm.weight"], wm[p + "rnn.layer_norm.bias"], eps)
+    x_pre = F.linear(torch.cat((z, a), -1), wm[p + "mlp._model.0.weight"])
+    x = F.silu(layer_norm(x_pre, wm[p + "mlp._model.1.weight"], wm[p + "mlp._model.1.bias"], eps))
+    g_pre = F.linear(torch.cat((h, x), -1), wm[p + "rnn.linear.weight"])
+    g = layer_norm(g_pre, wm[p + "rnn.layer_norm.weight"], wm[p + "rnn.layer_norm.bias"], eps)
+    if saves is not None:
+        saves.update(x_pre=x_pre, x_act=x, g_pre=g_pre, g_ln=g)
     r, c, u = torch.chunk(g, 3, -1)
     c = torch.tanh(torch.sigmoid(r) * c)
     u = torch.sigmoid(u - 1)

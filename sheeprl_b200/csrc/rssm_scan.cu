@@ -1336,13 +1336,13 @@ bool fixed_dims(const b200rl_rssm_scan_args& a) { return a.S == 32 && a.D == 32 
 int scan_check(const b200rl_rssm_scan_args& a) {
   RL_CHECK_ARG(a.B >= 1 && a.B <= MAXB, "persistent scan supports batch <= 16 rows per rank");
   RL_CHECK_ARG(a.D >= 1 && a.D <= 32, "persistent scan supports <= 32 classes per categorical");
-  RL_CHECK_ARG(a.T >= 1 && a.S >= 1 && a.S <= 64, "bad T / S (S <= 64)");
+  RL_CHECK_ARG(a.T >= 1 && a.S >= 1 && a.S <= 64, "persistent scan supports T >= 1 and 1 <= S <= 64 categoricals");
   RL_CHECK_ARG(a.Dx % 2 == 0 && a.R % 2 == 0 && a.Dr % 2 == 0 && (a.S * a.D) % 2 == 0, "persistent scan supports even layer widths");
-  RL_CHECK_ARG(a.Dx <= 4 * SCAN_NT, "persistent scan supports recurrent dense_units <= 1024");
+  // at most two 4-column groups of x_pre per CTA: the widest owned share the tests run (Dx = 1024)
+  RL_CHECK_ARG(a.Dx <= 1024, "persistent scan supports recurrent dense_units <= 1024");
   // one element of every per-step epilogue per thread (fixed assignments, rssm_scan.cu `Slot`)
-  RL_CHECK_ARG(MAXB * owned_groups(a.R, 0) * 12 <= SCAN_NT && MAXB * owned_groups(a.Dr, 0) * 4 <= SCAN_NT &&
-                   owned_groups(a.Dx, 0) <= 4,
-               "persistent scan supports recurrent_state_size <= 512 and hidden / dense sizes <= 2048");
+  RL_CHECK_ARG(MAXB * owned_groups(a.R, 0) * 12 <= SCAN_NT, "persistent scan supports recurrent_state_size <= 1024");
+  RL_CHECK_ARG(MAXB * owned_groups(a.Dr, 0) * 4 <= SCAN_NT, "persistent scan supports representation hidden_size <= 4096");
   RL_CHECK_ARG(a.workspace && a.workspace_bytes >= (long long)ws_bytes(a.T, a.B, a.S, a.D, a.Dx, a.R, a.Dr), "workspace too small");
   return B200RL_OK;
 }

@@ -157,15 +157,28 @@ def test_engine_cuda_full_size_properties():
     assert float((runs[0][0] - runs[1][0]).abs().max()) <= 2e-3 * float(runs[0][0].abs().max())
 
 
-@pytest.mark.parametrize("name", ["dv3_tiny_a", "dv3_tiny_b", "S"])
+SCAN_MODELS = {
+    "S": dict(size="S"),
+    "XS": dict(size="XS"),
+    # two 4-column groups per CTA in the GRU and x layers, forward and backward fused
+    "wide_mh2": dict(size="S", per_rank_sequence_length=6, horizon=3, dense_units=520, recurrent_state_size=520,
+                     hidden_size=64, stochastic_size=8, discrete_size=8, mlp_layers=1, cnn_channels_multiplier=4),
+    # the forward fits in shared memory, the backward does not: fused forward, per-step BPTT over its saves
+    "mixed_bwd": dict(size="S", per_rank_batch_size=8, per_rank_sequence_length=6, horizon=3, dense_units=128,
+                      recurrent_state_size=768, hidden_size=128, stochastic_size=16, discrete_size=16, mlp_layers=1,
+                      cnn_channels_multiplier=4),
+}
+
+
+@pytest.mark.parametrize("name", ["dv3_tiny_a", "dv3_tiny_b", "S", "XS", "wide_mh2", "mixed_bwd"])
 def test_fused_scan_equals_per_step_scan(name):
     """Persistent cooperative RSSM kernels (csrc/rssm_scan.cu, forward + BPTT) vs the per-step kernels:
     same saved activations, same world-model gradients."""
     from oracle import dv3_oracle as O
     from sheeprl_b200.configs import make_dv3_cfg
 
-    if name == "S":
-        cfg, adim = make_dv3_cfg("S"), (2,)
+    if name in SCAN_MODELS:
+        cfg, adim = make_dv3_cfg(**SCAN_MODELS[name]), (2,)
         wm, actor, critic, target = O.init_params(cfg, adim, seed=0)
         g = torch.Generator().manual_seed(3)
         for v in wm.values():
@@ -187,7 +200,10 @@ def test_fused_scan_equals_per_step_scan(name):
         torch.cuda.synchronize()
         if fused:
             assert eng.fused_scan, "fused scan was disabled"
-            assert eng.fused_scan_bwd or os.environ.get("B200RL_SCAN_BWD", "1") == "0", "fused backward scan was disabled"
+            if name == "mixed_bwd":
+                assert not eng.fused_scan_bwd, "the backward kernel should not fit this model"
+            else:
+                assert eng.fused_scan_bwd or os.environ.get("B200RL_SCAN_BWD", "1") == "0", "fused backward scan was disabled"
             assert eng.ops.rssm_scan_error(eng._scan_ws) == 0, "a hand-off of the persistent scan timed out"
         outs.append({k: getattr(eng, k).clone() for k in (
             "latent", "z_in", "h_in", "a_in", "x_pre", "x_act", "g_pre", "g_ln", "tr_pre", "tr_act", "rp_pre", "rp_act",
