@@ -39,7 +39,9 @@ int b200rl_gemm_f32(const float* A, const float* B, float* C, const float* bias,
 /* Precision of every tensor-core product (GEMM, conv forward / input gradient / weight gradient), process-wide like
  * torch.set_float32_matmul_precision (the reference sets it from configs/config.yaml:18, default "high"):
  * 3 = three TF32 products per k-step on x = hi + lo (fp32-accurate, default; the 1e-4 parity tests run this),
- * 1 = one TF32 product ("high": the numerics of the reference's own GPU runs, ~3x the throughput). */
+ * 1 = one TF32 product ("high": the numerics of the reference's own GPU runs, ~3x the throughput).
+ * Every tensor-core route (GEMM layouts, split-K, gemm_ln, conv down / up, both weight-gradient routes) is checked in
+ * both precisions against a float64 reference (tests/test_gpu_tc_precision.py). */
 int b200rl_set_matmul_precision(int tf32_passes);
 int b200rl_get_matmul_precision(void);
 int b200rl_gemm_tc_supported(const float* A, const float* B, int M, int N, int K, int lda, int ldb, int transA,
