@@ -215,6 +215,12 @@ int b200rl_sumsq(const float* x, long long n, double* out, cudaStream_t stream);
 int b200rl_adam_step(float* p, const float* g, float* m, float* v, const double* normsq, const int* step_dev,
                      float* norm_out, long long n, float max_norm, float lr, float b1, float b2, float eps,
                      cudaStream_t stream);
+/* fabric.clip_gradients + torch.optim.RMSprop.step (single-tensor path; A2C, a2c/a2c.py:102-105) in one pass, with
+ * adam_step's normsq / norm_out contract.  square_avg always; momentum_buf read and written only when momentum > 0;
+ * grad_avg non-NULL selects `centered`.  eps is added after the square root; the step count does not enter the update. */
+int b200rl_rmsprop_step(float* p, const float* g, float* square_avg, float* momentum_buf, float* grad_avg,
+                        const double* normsq, float* norm_out, long long n, float max_norm, float lr, float alpha,
+                        float eps, float weight_decay, float momentum, cudaStream_t stream);
 int b200rl_ema(float* target, const float* src, long long n, float tau, cudaStream_t stream);
 int b200rl_fill_exponential(float* out, long long n, unsigned long long seed, unsigned int stream_id,
                             const int* counter_dev, cudaStream_t stream);
@@ -301,6 +307,16 @@ int b200rl_ppo_loss_masked(const float* head, const float* actions, const float*
                            float* dhead, float* dvalues, float* losses, int B, const int* head_dims, int n_heads,
                            int is_continuous, int clip_vloss, int normalize_adv, float clip_coef, float vf_coef,
                            float ent_coef, cudaStream_t stream);
+/* A2C objective (a2c/a2c.py:60-100, a2c/loss.py, ppo/loss.py:44-75) of every minibatch of a rollout in one launch,
+ * one CTA per minibatch.  Rows are the gathered rollout in sampler order; minibatch i is rows [i*seg, min(N, (i+1)*seg))
+ * (the last one may be short).  Per minibatch: optional advantage normalisation (unbiased std + 1e-8), policy
+ * -(logp*adv), value (value - return)^2 and entropy -entropy losses reduced by mean (reduce_sum 0) or sum (1);
+ * dhead / dvalues = gradient of policy + vf_coef*value + ent_coef*entropy of the row's own minibatch; losses[n_seg, 3].
+ * Distributions as b200rl_ppo_loss.  normalize_adv needs at least two rows in every minibatch. */
+int b200rl_a2c_loss(const float* head, const float* actions, const float* adv, const float* values, const float* returns,
+                    float* dhead, float* dvalues, float* losses, int N, int seg, const int* head_dims, int n_heads,
+                    int is_continuous, int normalize_adv, int reduce_sum, float vf_coef, float ent_coef,
+                    cudaStream_t stream);
 /* Single-layer LSTM over padded time-major sequences in one launch (recurrent PPO, ppo_recurrent/agent.py:67-80; torch
  * gate order i, f, g, o).  xw [T, B, 4H] = x W_ih^T + b_ih + b_hh; W_hh [4H, H]; h0, c0 [B, H]; lengths [B] int32 in
  * [1, T] (sequence b is valid for t < lengths[b]).  out [T, B, H] (0 at padded steps); gates [T, B, 4H] (activated)

@@ -144,6 +144,10 @@ class PPOPlayer:
     def actor(self):
         return PPOPlayer._ActorInfo(self.engine)
 
+    def eval(self):
+        """the reference's test() puts the player in eval mode first (ppo/utils.py:41); there is nothing to switch"""
+        return self
+
     def _run(self, obs, actor: bool, critic: bool):
         e, s = self.engine, self.engine.spec
         rgb, x_state = gather_obs(s, obs)

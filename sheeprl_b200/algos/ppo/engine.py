@@ -174,6 +174,11 @@ class PPOEngine:
 
     def load_reference_state(self, state: Dict[str, torch.Tensor]):
         """reference PPOAgent.state_dict() keys/shapes ('_forward_module.' infixes of Fabric wrappers are ignored)"""
+        self.group.load(self.internal_state(state))
+
+    def internal_state(self, state: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+        """tensors in the reference's keys / shapes -> the flat group's names / layouts (the inverse of
+        export_reference_state; also used for optimizer state, which has the parameters' layout)"""
         st = {k.replace("_forward_module.", ""): v for k, v in state.items()}
         want = self.reference_shapes()
         missing, extra = set(want) - set(st), set(st) - set(want)
@@ -193,7 +198,7 @@ class PPOEngine:
                 internal[k] = torch.cat([st[f"actor.actor_heads.{i}.bias"] for i in range(len(heads))], 0)
             else:
                 internal[k] = st[k]
-        self.group.load(internal)
+        return internal
 
     def export_reference_state(self, views=None) -> "OrderedDict[str, torch.Tensor]":
         views = self.group.views if views is None else views
@@ -323,7 +328,6 @@ class PPOEngine:
             return out
 
         # ---- forward
-        feat = b["feat"]
         x_state = rows("state").unsqueeze(0) if s["mlp_dim"] else None
         self.forward(b, rows("rgb") if self.geo else None, x_state)
         # ---- objective + gradients w.r.t. head outputs and values
@@ -331,8 +335,14 @@ class PPOEngine:
                    b["values"].reshape(-1), rows("values").reshape(-1), rows("returns").reshape(-1), b["dhead"][0],
                    b["dvalues"].reshape(-1), self.losses, self.head_dims, self.dist_mode, hp["clip_vloss"],
                    hp["normalize_advantages"], hp["clip_coef"], hp["vf_coef"], hp["ent_coef"])
-        # ---- backward: actor, critic -> feature gradient (cnn columns masked by the fc ReLU)
-        F_ = self.F
+        self._backward(b, x_state)
+        self._optimizer_step()
+
+    def _backward(self, b: dict, x_state):
+        """every weight gradient from b["dhead"] / b["dvalues"] (the objective's output) down to the encoders; each
+        product reduces over all rows of `b`"""
+        o, F_, feat = self.ops, self.F, b["feat"]
+        # actor, critic -> feature gradient (cnn columns masked by the fc ReLU)
         for j, (st, dout) in enumerate(((self.actor, b["dhead"]), (self.critic, b["dvalues"]))):
             dpre0, l0 = self._mlp_bwd(st, b, dout), st.lins[0]
             o.bgemm(dpre0.transpose(1, 2), feat, l0.gW, rsum=l0.gb)
@@ -341,7 +351,6 @@ class PPOEngine:
             if self.Mf:
                 o.bgemm(dpre0, l0.W[:, :, F_:], b["dfeat"][:, :, F_:], accumulate=j > 0)
         self._encoder_bwd(b, x_state)
-        self._optimizer_step()
 
     def _encoder_bwd(self, b: dict, x_state):
         """weight gradients of the vector and image encoders from b["dfeat"] (its image columns already masked by the
@@ -374,9 +383,13 @@ class PPOEngine:
         o.increment(g.step_t)
         g.step += 1
         handle = getattr(g, "optimizer", None)              # B200Adam: the reference's PolynomialLR edits its param_groups
-        lr = handle.lr if handle is not None else self.opt["lr"]
-        o.adam_step(g.flat, g.grad, g.exp_avg, g.exp_avg_sq, self.normsq, float(hp["max_grad_norm"]), lr,
-                    self.opt["betas"][0], self.opt["betas"][1], self.opt["eps"], g.step_t, self.norm_out)
+        self._apply_update(handle.lr if handle is not None else self.opt["lr"])
+
+    def _apply_update(self, lr: float):
+        """the fused clip + optimizer update of the flat group (gradient norm already in self.normsq)"""
+        g = self.group
+        self.ops.adam_step(g.flat, g.grad, g.exp_avg, g.exp_avg_sq, self.normsq, float(self.hp["max_grad_norm"]), lr,
+                           self.opt["betas"][0], self.opt["betas"][1], self.opt["eps"], g.step_t, self.norm_out)
 
     def train(self, data: Dict[str, torch.Tensor], index_batches: Sequence[Sequence[int]], on_minibatch=None):
         for ib in index_batches:

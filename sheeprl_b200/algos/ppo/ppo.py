@@ -22,8 +22,9 @@ def make_optimizer(agent, cfg=None) -> B200Adam:
     return B200Adam(e.group, list(e.group.shapes), e.opt["lr"], e.opt["eps"], e.opt["betas"])
 
 
-def minibatch_indices(n_rows: int, fabric, cfg):
-    """The reference's sampler stack (ppo.py:39-56), yielding one list of row indices per minibatch."""
+def minibatch_indices(n_rows: int, fabric, cfg, epochs: Optional[int] = None):
+    """The reference's sampler stack (ppo.py:39-56), yielding one list of row indices per minibatch over `epochs`
+    passes (default cfg.algo.update_epochs; A2C makes one, a2c.py:40-55)."""
     indexes = list(range(n_rows))
     if cfg.buffer.share_data:
         sampler = DistributedSampler(indexes, num_replicas=fabric.world_size, rank=fabric.global_rank, shuffle=True,
@@ -31,7 +32,7 @@ def minibatch_indices(n_rows: int, fabric, cfg):
     else:
         sampler = RandomSampler(indexes)
     batches = BatchSampler(sampler, batch_size=cfg.algo.per_rank_batch_size, drop_last=False)
-    for epoch in range(cfg.algo.update_epochs):
+    for epoch in range(cfg.algo.update_epochs if epochs is None else epochs):
         if cfg.buffer.share_data:
             batches.sampler.set_epoch(epoch)
         yield from batches

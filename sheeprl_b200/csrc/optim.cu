@@ -1,7 +1,8 @@
 // Optimiser + small utility kernels on the flat parameter groups (pure HBM streaming).
 //
 // Replaces (reference): fabric.clip_gradients -> torch.nn.utils.clip_grad_norm_ and torch.optim.Adam.step
-// (dreamer_v3.py:191-200, :298-304, :318-327; configs/optim/adam.yaml), the per-parameter target-critic EMA
+// (dreamer_v3.py:191-200, :298-304, :318-327; configs/optim/adam.yaml), torch.optim.RMSprop.step (a2c/a2c.py:102-105;
+// configs/optim/rmsprop.yaml), the per-parameter target-critic EMA
 // loop (dreamer_v3.py:674-680), torch.multinomial's Exp(1) noise (Philox4x32-10 here).
 // Clip + Adam are one pass: 4 reads + 3 writes of 4 B per parameter = 28 B/param (SURVEY.md §8d).
 #include "common.cuh"
@@ -86,6 +87,84 @@ adam_step_kernel(float* __restrict__ p, const float* __restrict__ g, float* __re
     p[i] = pi;
     m[i] = mi;
     v[i] = vi;
+  }
+}
+
+// One element of clip + torch.optim.RMSprop (single-tensor path, torch/optim/rmsprop.py).  Unlike Adam, eps is added
+// AFTER the square root, and the step count does not enter the update.
+template <bool CENTERED, bool MOMENTUM>
+__device__ __forceinline__ void rmsprop_update(float& p, float g, float& sq, float& buf, float& gavg, float coef,
+                                               float lr, float alpha, float eps, float weight_decay, float momentum) {
+  g *= coef;
+  if (weight_decay != 0.f) g = g + weight_decay * p;               // grad.add(param, alpha=weight_decay)
+  sq = sq * alpha + (1.f - alpha) * g * g;                          // square_avg.mul_(alpha).addcmul_(grad, grad, 1-alpha)
+  float avg;
+  if (CENTERED) {
+    gavg = gavg + (1.f - alpha) * (g - gavg);                       // grad_avg.lerp_(grad, 1 - alpha)
+    avg = sqrtf(sq - gavg * gavg) + eps;
+  } else {
+    avg = sqrtf(sq) + eps;
+  }
+  if (MOMENTUM) {
+    buf = buf * momentum + g / avg;                                 // buf.mul_(momentum).addcdiv_(grad, avg)
+    p = p - lr * buf;
+  } else {
+    p = p - lr * (g / avg);
+  }
+}
+
+// sq = square_avg; buf = momentum_buffer (touched only when MOMENTUM); gavg = grad_avg (only when CENTERED)
+template <bool CENTERED, bool MOMENTUM>
+__global__ void __launch_bounds__(256)
+rmsprop_step_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ sq, float* __restrict__ buf,
+                    float* __restrict__ gavg, const double* __restrict__ normsq, float* __restrict__ norm_out,
+                    long long n, float max_norm, float lr, float alpha, float eps, float weight_decay, float momentum,
+                    int vec) {
+  __shared__ float s_coef;
+  if (threadIdx.x == 0) {
+    const float total = (float)sqrt(*normsq);
+    float coef = 1.f;
+    if (max_norm > 0.f) coef = fminf(max_norm / (total + 1e-6f), 1.f);
+    s_coef = coef;
+    if (blockIdx.x == 0) norm_out[0] = total;
+  }
+  __syncthreads();
+  const float coef = s_coef;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  long long done = 0;
+  if (vec) {   // 128-bit accesses (flat groups are 256-byte aligned)
+    const long long n4 = n >> 2;
+    float4* p4 = reinterpret_cast<float4*>(p);
+    const float4* g4 = reinterpret_cast<const float4*>(g);
+    float4* s4 = reinterpret_cast<float4*>(sq);
+    float4* b4 = reinterpret_cast<float4*>(buf);
+    float4* a4 = reinterpret_cast<float4*>(gavg);
+    for (long long i = tid; i < n4; i += stride) {
+      float4 pp = p4[i], ss = s4[i];
+      const float4 gg = g4[i];
+      float4 bb = make_float4(0.f, 0.f, 0.f, 0.f), aa = bb;
+      if (MOMENTUM) bb = b4[i];
+      if (CENTERED) aa = a4[i];
+      rmsprop_update<CENTERED, MOMENTUM>(pp.x, gg.x, ss.x, bb.x, aa.x, coef, lr, alpha, eps, weight_decay, momentum);
+      rmsprop_update<CENTERED, MOMENTUM>(pp.y, gg.y, ss.y, bb.y, aa.y, coef, lr, alpha, eps, weight_decay, momentum);
+      rmsprop_update<CENTERED, MOMENTUM>(pp.z, gg.z, ss.z, bb.z, aa.z, coef, lr, alpha, eps, weight_decay, momentum);
+      rmsprop_update<CENTERED, MOMENTUM>(pp.w, gg.w, ss.w, bb.w, aa.w, coef, lr, alpha, eps, weight_decay, momentum);
+      p4[i] = pp;
+      s4[i] = ss;
+      if (MOMENTUM) b4[i] = bb;
+      if (CENTERED) a4[i] = aa;
+    }
+    done = n4 << 2;
+  }
+  for (long long i = done + tid; i < n; i += stride) {
+    float pi = p[i], si = sq[i];
+    float bi = MOMENTUM ? buf[i] : 0.f, ai = CENTERED ? gavg[i] : 0.f;
+    rmsprop_update<CENTERED, MOMENTUM>(pi, g[i], si, bi, ai, coef, lr, alpha, eps, weight_decay, momentum);
+    p[i] = pi;
+    sq[i] = si;
+    if (MOMENTUM) buf[i] = bi;
+    if (CENTERED) gavg[i] = ai;
   }
 }
 
@@ -240,6 +319,26 @@ extern "C" int b200rl_adam_step(float* p, const float* g, float* m, float* v, co
                     reinterpret_cast<uintptr_t>(v)) & 15) == 0;
   adam_step_kernel<<<stream_grid(vec ? (n + 3) / 4 : n), 256, 0, st>>>(p, g, m, v, normsq, step_t, norm_out, n, max_norm, lr,
                                                                       b1, b2, eps, vec);
+  RL_CHECK_LAUNCH();
+  return B200RL_OK;
+}
+
+extern "C" int b200rl_rmsprop_step(float* p, const float* g, float* square_avg, float* momentum_buf, float* grad_avg,
+                                   const double* normsq, float* norm_out, long long n, float max_norm, float lr,
+                                   float alpha, float eps, float weight_decay, float momentum, cudaStream_t st) {
+  RL_CHECK_ARG(p && g && square_avg && normsq && norm_out, "null pointer");
+  RL_CHECK_ARG(momentum <= 0.f || momentum_buf, "momentum > 0 needs the momentum buffer");
+  if (n <= 0) return B200RL_OK;
+  const int vec = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) |
+                    reinterpret_cast<uintptr_t>(square_avg) |
+                    reinterpret_cast<uintptr_t>(momentum > 0.f ? momentum_buf : nullptr) |
+                    reinterpret_cast<uintptr_t>(grad_avg)) & 15) == 0;
+  const int grid = stream_grid(vec ? (n + 3) / 4 : n);
+  const bool centered = grad_avg != nullptr, mom = momentum > 0.f;
+  auto k = centered ? (mom ? rmsprop_step_kernel<true, true> : rmsprop_step_kernel<true, false>)
+                    : (mom ? rmsprop_step_kernel<false, true> : rmsprop_step_kernel<false, false>);
+  k<<<grid, 256, 0, st>>>(p, g, square_avg, momentum_buf, grad_avg, normsq, norm_out, n, max_norm, lr, alpha, eps,
+                          weight_decay, momentum, vec);
   RL_CHECK_LAUNCH();
   return B200RL_OK;
 }

@@ -5,7 +5,7 @@
 // (sheeprl/models/models.py:288-328, cnn_forward utils/model.py:165-223), PPOAgent.forward's distribution glue
 // (OneHotCategorical / Independent(Normal) log_prob + entropy, sheeprl/algos/ppo/agent.py:179-239),
 // normalize_tensor (utils/utils.py:121-130) and policy_loss / value_loss / entropy_loss (ppo/loss.py:6-75) with
-// their autograd backward.
+// their autograd backward; A2C's objective (a2c/a2c.py:60-100, a2c/loss.py) over every minibatch of a rollout.
 //
 // Convolutions are channel-last: rows of the patch matrix are output pixels (b, oy, ox), columns are (ky, kx, c), so
 // a conv is patch-gather -> product with the [Cout, k, k, Cin] weight (stored in that layout in the flat parameter
@@ -82,6 +82,81 @@ struct PpoLossArgs {
   float clip_coef, vf_coef, ent_coef;
 };
 
+// ---- per-row distribution math shared by the PPO and A2C objectives (ppo/agent.py:179-239).  hd: the row's head
+// outputs (`width` floats); act: the row's stored action (one-hot [width] when discrete, [width / 2] when continuous).
+// Log-probability of the taken action and entropy of the row's distribution.
+__device__ __forceinline__ void row_logp_entropy(const float* hd, const float* act, int width, int n_heads,
+                                                 const int* head_dims, int is_continuous, float& lp, float& ent) {
+  lp = 0.f;
+  ent = 0.f;
+  if (is_continuous) {
+    const int A = width / 2;
+    float corr = 0.f;
+    for (int j = 0; j < A; ++j) {
+      float x = act[j];
+      if (is_continuous == 2) { corr += tanh_logp_term(x); x = safe_atanh(x); }
+      const float mu = hd[j], ls = hd[A + j], sd = expf(ls), d = x - mu;
+      lp += -(d * d) / (2.f * sd * sd) - ls - 0.9189385332046727f;
+      ent += 0.5f + 0.9189385332046727f + ls;
+    }
+    lp -= corr;
+  } else {
+    int off = 0;
+    for (int h = 0; h < n_heads; ++h) {
+      const int n = head_dims[h];
+      float m = -INFINITY;
+      for (int j = 0; j < n; ++j) m = fmaxf(m, hd[off + j]);
+      float z = 0.f;
+      for (int j = 0; j < n; ++j) z += expf(hd[off + j] - m);
+      const float lse = m + logf(z);
+      float hh = 0.f;
+      for (int j = 0; j < n; ++j) {
+        const float lpj = hd[off + j] - lse;
+        lp += lpj * act[off + j];
+        hh -= expf(lpj) * lpj;
+      }
+      ent += hh;
+      off += n;
+    }
+  }
+}
+
+// dh = dlp * d(logp)/d(head) + dent * d(entropy)/d(head) for one row
+__device__ __forceinline__ void row_head_grad(const float* hd, const float* act, float* dh, int width, int n_heads,
+                                              const int* head_dims, int is_continuous, float dlp, float dent) {
+  if (is_continuous) {
+    const int A = width / 2;
+    for (int j = 0; j < A; ++j) {
+      float x = act[j];
+      if (is_continuous == 2) x = safe_atanh(x);             // the squash term does not depend on the head
+      const float mu = hd[j], ls = hd[A + j], sd = expf(ls), d = x - mu;
+      dh[j] = dlp * d / (sd * sd);
+      dh[A + j] = dlp * (d * d / (sd * sd) - 1.f) + dent;
+    }
+  } else {
+    int off = 0;
+    for (int h = 0; h < n_heads; ++h) {
+      const int n = head_dims[h];
+      float m = -INFINITY;
+      for (int j = 0; j < n; ++j) m = fmaxf(m, hd[off + j]);
+      float z = 0.f;
+      for (int j = 0; j < n; ++j) z += expf(hd[off + j] - m);
+      const float lse = m + logf(z);
+      float hh = 0.f, asum = 0.f;
+      for (int j = 0; j < n; ++j) {
+        const float lpj = hd[off + j] - lse;
+        hh -= expf(lpj) * lpj;
+        asum += act[off + j];
+      }
+      for (int j = 0; j < n; ++j) {
+        const float lpj = hd[off + j] - lse, pj = expf(lpj);
+        dh[off + j] = dlp * (act[off + j] - pj * asum) - dent * pj * (lpj + hh);
+      }
+      off += n;
+    }
+  }
+}
+
 // One CTA: B is a minibatch (<= a few thousand rows).  MASKED (ppo_recurrent.py:77-101): only rows with
 // mask != 0 count; the means are over their number n, advantages are normalised over them when n > 1, and the other
 // rows get zero gradients.
@@ -112,48 +187,21 @@ __global__ void __launch_bounds__(256) ppo_loss_kernel(const PpoLossArgs a) {
   }
   int width = 0;
   for (int h = 0; h < a.n_heads; ++h) width += a.head_dims[h];
+  const int A = width;
   if (a.is_continuous) width *= 2;
+  const int act_w = a.is_continuous ? A : width;
   float s_pg = 0.f, s_v = 0.f, s_e = 0.f;
   for (int b = threadIdx.x; b < B; b += blockDim.x) {
     const float* hd = a.head + (long long)b * width;
+    const float* act = a.actions + (long long)b * act_w;
     float* dh = a.dhead + (long long)b * width;
     if (MASKED && a.mask[b] == 0.f) {
       for (int j = 0; j < width; ++j) dh[j] = 0.f;
       a.dvalues[b] = 0.f;
       continue;
     }
-    float lp = 0.f, ent = 0.f;
-    // ---- pass 1: log-prob of the taken action and entropy (ppo/agent.py:179-239)
-    if (a.is_continuous) {
-      const int A = width / 2;
-      float corr = 0.f;
-      for (int j = 0; j < A; ++j) {
-        float x = a.actions[(long long)b * A + j];
-        if (a.is_continuous == 2) { corr += tanh_logp_term(x); x = safe_atanh(x); }
-        const float mu = hd[j], ls = hd[A + j], sd = expf(ls), d = x - mu;
-        lp += -(d * d) / (2.f * sd * sd) - ls - 0.9189385332046727f;
-        ent += 0.5f + 0.9189385332046727f + ls;
-      }
-      lp -= corr;
-    } else {
-      int off = 0;
-      for (int h = 0; h < a.n_heads; ++h) {
-        const int n = a.head_dims[h];
-        float m = -INFINITY;
-        for (int j = 0; j < n; ++j) m = fmaxf(m, hd[off + j]);
-        float z = 0.f;
-        for (int j = 0; j < n; ++j) z += expf(hd[off + j] - m);
-        const float lse = m + logf(z);
-        float hh = 0.f;
-        for (int j = 0; j < n; ++j) {
-          const float lpj = hd[off + j] - lse;
-          lp += lpj * a.actions[(long long)b * width + off + j];
-          hh -= expf(lpj) * lpj;
-        }
-        ent += hh;
-        off += n;
-      }
-    }
+    float lp, ent;
+    row_logp_entropy(hd, act, width, a.n_heads, a.head_dims, a.is_continuous, lp, ent);
     // ---- objective (ppo/loss.py) and d/dlp, d/dent, d/dvalue
     const float adv = (a.adv[b] - mean) * inv_std;
     const float ratio = expf(lp - a.old_logp[b]);
@@ -179,38 +227,7 @@ __global__ void __launch_bounds__(256) ppo_loss_kernel(const PpoLossArgs a) {
     a.dvalues[b] = a.vf_coef * dval * invB;
     s_e += -ent;
     const float dent = -a.ent_coef * invB;
-    // ---- pass 2: gradient w.r.t. the head outputs
-    if (a.is_continuous) {
-      const int A = width / 2;
-      for (int j = 0; j < A; ++j) {
-        float x = a.actions[(long long)b * A + j];
-        if (a.is_continuous == 2) x = safe_atanh(x);             // the squash term does not depend on the head
-        const float mu = hd[j], ls = hd[A + j], sd = expf(ls), d = x - mu;
-        dh[j] = dlp * d / (sd * sd);
-        dh[A + j] = dlp * (d * d / (sd * sd) - 1.f) + dent;
-      }
-    } else {
-      int off = 0;
-      for (int h = 0; h < a.n_heads; ++h) {
-        const int n = a.head_dims[h];
-        float m = -INFINITY;
-        for (int j = 0; j < n; ++j) m = fmaxf(m, hd[off + j]);
-        float z = 0.f;
-        for (int j = 0; j < n; ++j) z += expf(hd[off + j] - m);
-        const float lse = m + logf(z);
-        float hh = 0.f, asum = 0.f;
-        for (int j = 0; j < n; ++j) {
-          const float lpj = hd[off + j] - lse;
-          hh -= expf(lpj) * lpj;
-          asum += a.actions[(long long)b * width + off + j];
-        }
-        for (int j = 0; j < n; ++j) {
-          const float lpj = hd[off + j] - lse, pj = expf(lpj);
-          dh[off + j] = dlp * (a.actions[(long long)b * width + off + j] - pj * asum) - dent * pj * (lpj + hh);
-        }
-        off += n;
-      }
-    }
+    row_head_grad(hd, act, dh, width, a.n_heads, a.head_dims, a.is_continuous, dlp, dent);
   }
   s_pg = block_sum(s_pg, red);
   s_v = block_sum(s_v, red);
@@ -219,6 +236,73 @@ __global__ void __launch_bounds__(256) ppo_loss_kernel(const PpoLossArgs a) {
     a.losses[0] = s_pg * invB;
     a.losses[1] = s_v * invB;
     a.losses[2] = s_e * invB;
+  }
+}
+
+struct A2cLossArgs {
+  const float* head; const float* actions; const float* adv; const float* values; const float* returns;
+  float* dhead; float* dvalues; float* losses;   // losses[n_seg, 3] = policy, value, entropy
+  int N, seg, n_heads; int head_dims[8];
+  int is_continuous, normalize_adv, reduce_sum;
+  float vf_coef, ent_coef;
+};
+
+// A2C objective (a2c/a2c.py:60-100, a2c/loss.py, ppo/loss.py:44-75) of every minibatch of a rollout in one launch.
+// The rows are the gathered rollout in sampler order; CTA i owns minibatch i = rows [i*seg, min(N, (i+1)*seg)).
+// Per minibatch: optional advantage normalisation over its rows, pg = -(logp*adv), v = (value - return)^2,
+// ent = -entropy, each reduced by `mean` (scale 1/rows) or `sum` (scale 1); the gradient of
+// pg + vf_coef*v + ent_coef*ent of every minibatch lands on its own rows, so one backward over all N rows gives the
+// sum of the per-minibatch gradients the reference accumulates.
+__global__ void __launch_bounds__(256) a2c_loss_kernel(const A2cLossArgs a) {
+  __shared__ float red[32];
+  __shared__ int dims[8];                                  // indexed per head: kept out of the parameter struct
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int h = 0; h < 8; ++h) dims[h] = a.head_dims[h];
+  }
+  __syncthreads();
+  const int r0 = blockIdx.x * a.seg;
+  const int n = min(a.N - r0, a.seg);
+  const float scale = a.reduce_sum ? 1.f : 1.f / (float)n;
+  float mean = 0.f, inv_std = 1.f;
+  if (a.normalize_adv) {                                   // utils/utils.py:121-130 over this minibatch
+    float s = 0.f;
+    for (int b = r0 + threadIdx.x; b < r0 + n; b += blockDim.x) s += a.adv[b];
+    mean = block_sum(s, red) / (float)n;
+    float v = 0.f;
+    for (int b = r0 + threadIdx.x; b < r0 + n; b += blockDim.x) { const float d = a.adv[b] - mean; v += d * d; }
+    v = block_sum(v, red) / (float)(n - 1);
+    inv_std = 1.f / (sqrtf(v) + 1e-8f);
+  }
+  int width = 0;
+  for (int h = 0; h < a.n_heads; ++h) width += dims[h];
+  const int A = width;
+  if (a.is_continuous) width *= 2;
+  const int act_w = a.is_continuous ? A : width;
+  const float dent = -a.ent_coef * scale;
+  float s_pg = 0.f, s_v = 0.f, s_e = 0.f;
+  for (int b = r0 + threadIdx.x; b < r0 + n; b += blockDim.x) {
+    const float* hd = a.head + (long long)b * width;
+    const float* act = a.actions + (long long)b * act_w;
+    float lp, ent;
+    row_logp_entropy(hd, act, width, a.n_heads, dims, a.is_continuous, lp, ent);
+    const float adv = (a.adv[b] - mean) * inv_std;
+    s_pg += -(lp * adv);
+    const float val = a.values[b], ret = a.returns[b];
+    s_v += (val - ret) * (val - ret);
+    a.dvalues[b] = a.vf_coef * 2.f * (val - ret) * scale;
+    s_e += -ent;
+    row_head_grad(hd, act, a.dhead + (long long)b * width, width, a.n_heads, dims, a.is_continuous,
+                  -adv * scale, dent);
+  }
+  s_pg = block_sum(s_pg, red);
+  s_v = block_sum(s_v, red);
+  s_e = block_sum(s_e, red);
+  if (threadIdx.x == 0) {
+    float* l = a.losses + 3 * (long long)blockIdx.x;
+    l[0] = s_pg * scale;
+    l[1] = s_v * scale;
+    l[2] = s_e * scale;
   }
 }
 
@@ -347,6 +431,28 @@ extern "C" int b200rl_ppo_loss_masked(const float* head, const float* actions, c
   a.is_continuous = is_continuous; a.clip_vloss = clip_vloss; a.normalize_adv = normalize_adv;
   a.clip_coef = clip_coef; a.vf_coef = vf_coef; a.ent_coef = ent_coef;
   ppo_loss_kernel<true><<<1, 256, 0, st>>>(a);
+  RL_CHECK_LAUNCH();
+  return B200RL_OK;
+}
+
+extern "C" int b200rl_a2c_loss(const float* head, const float* actions, const float* adv, const float* values,
+                               const float* returns, float* dhead, float* dvalues, float* losses, int N, int seg,
+                               const int* head_dims, int n_heads, int is_continuous, int normalize_adv, int reduce_sum,
+                               float vf_coef, float ent_coef, cudaStream_t st) {
+  RL_CHECK_ARG(head && actions && adv && values && returns && dhead && dvalues && losses && head_dims, "null pointer");
+  RL_CHECK_ARG(N > 0 && seg > 0 && n_heads > 0 && n_heads <= 8, "bad dims (at most 8 action heads)");
+  RL_CHECK_ARG(is_continuous >= 0 && is_continuous <= 2, "is_continuous: 0 discrete, 1 normal, 2 tanh_normal");
+  const long long n_seg = ((long long)N + seg - 1) / seg;
+  RL_CHECK_ARG(!normalize_adv || (seg > 1 && N - (n_seg - 1) * seg > 1),
+               "advantage normalisation needs at least two rows in every minibatch");
+  A2cLossArgs a{};
+  a.head = head; a.actions = actions; a.adv = adv; a.values = values; a.returns = returns;
+  a.dhead = dhead; a.dvalues = dvalues; a.losses = losses;
+  a.N = N; a.seg = seg; a.n_heads = n_heads;
+  for (int i = 0; i < n_heads; ++i) a.head_dims[i] = head_dims[i];
+  a.is_continuous = is_continuous; a.normalize_adv = normalize_adv; a.reduce_sum = reduce_sum;
+  a.vf_coef = vf_coef; a.ent_coef = ent_coef;
+  a2c_loss_kernel<<<(unsigned)n_seg, 256, 0, st>>>(a);
   RL_CHECK_LAUNCH();
   return B200RL_OK;
 }

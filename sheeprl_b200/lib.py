@@ -405,6 +405,18 @@ class CudaOps:
                                            c_ll(p.numel()), c_float(max_norm), c_float(lr), c_float(b1), c_float(b2),
                                            c_float(eps), self._st()))
 
+    def rmsprop_step(self, p, g, square_avg, momentum_buf, grad_avg, normsq, max_norm, lr, alpha, eps, weight_decay,
+                     momentum, norm_out):
+        """clip + torch.optim.RMSprop; momentum_buf is used when momentum > 0, grad_avg (not None) selects centered"""
+        _f32(p, g, square_avg, momentum_buf, grad_avg, norm_out)
+        assert normsq.dtype == torch.float64
+        for t in (g, square_avg, momentum_buf, grad_avg):
+            assert t is None or t.numel() == p.numel()
+        self._ck(self.lib.b200rl_rmsprop_step(_p(p), _p(g), _p(square_avg), _p(momentum_buf), _p(grad_avg), _p(normsq),
+                                              _p(norm_out), c_ll(p.numel()), c_float(max_norm), c_float(lr),
+                                              c_float(alpha), c_float(eps), c_float(weight_decay), c_float(momentum),
+                                              self._st()))
+
     def ema(self, target, src, tau: float):
         _f32(target, src)
         self._ck(self.lib.b200rl_ema(_p(target), _p(src), c_ll(target.numel()), c_float(tau), self._st()))
@@ -649,6 +661,20 @@ class CudaOps:
                                                  c_int(int(is_continuous)), c_int(int(clip_vloss)),
                                                  c_int(int(normalize_adv)), c_float(clip_coef), c_float(vf_coef),
                                                  c_float(ent_coef), self._st()))
+
+    def a2c_loss(self, head, actions, adv, values, returns, dhead, dvalues, losses, seg: int, head_dims,
+                 is_continuous: int, normalize_adv: bool, reduce_sum: bool, vf_coef: float, ent_coef: float):
+        """A2C objective of every minibatch (rows [i*seg, min(N, (i+1)*seg))) of a rollout; losses [n_seg, 3]"""
+        _f32(head, actions, adv, values, returns, dhead, dvalues, losses)
+        for t in (head, actions, adv, values, returns, dhead, dvalues, losses):
+            assert t.is_contiguous()
+        N = head.shape[0]
+        assert losses.numel() == 3 * ((N + seg - 1) // seg)
+        dims = (c_int * len(head_dims))(*head_dims)
+        self._ck(self.lib.b200rl_a2c_loss(_p(head), _p(actions), _p(adv), _p(values), _p(returns), _p(dhead),
+                                          _p(dvalues), _p(losses), c_int(N), c_int(seg), dims, c_int(len(head_dims)),
+                                          c_int(int(is_continuous)), c_int(int(normalize_adv)), c_int(int(reduce_sum)),
+                                          c_float(vf_coef), c_float(ent_coef), self._st()))
 
     # ------------------------------------------------------------------ recurrent PPO: LSTM sequences (csrc/lstm.cu)
     def lstm_seq_fwd(self, xw, W_hh, h0, c0, lengths, out, gates=None, cs=None, hT=None, cT=None):

@@ -36,6 +36,7 @@ class FlatGroup:
             self.exp_avg = torch.zeros_like(self.flat)
             self.exp_avg_sq = torch.zeros_like(self.flat)
             self.gviews = self._views(self.grad)
+        self.grad_avg = None                                              # RMSprop(centered=True) only: alloc_grad_avg()
         self.step = 0                                                     # host mirror of step_t
         self.step_t = torch.zeros(1, dtype=torch.int32, device=device)    # device-side Adam step (graph-safe)
 
@@ -64,3 +65,9 @@ class FlatGroup:
 
     def optimizer_views(self):
         return self._views(self.exp_avg), self._views(self.exp_avg_sq)
+
+    def alloc_grad_avg(self) -> torch.Tensor:
+        """the one optimizer buffer not every group needs (centered RMSprop's grad_avg), allocated on first use"""
+        if self.grad_avg is None:
+            self.grad_avg = torch.zeros_like(self.flat)
+        return self.grad_avg
