@@ -30,7 +30,9 @@ int b200rl_device_check(void);
 /* ---- dense layers ------------------------------------------------------------------------------
  * nn.Linear forward/backward everywhere in sheeprl/models/models.py:16-119 (MLP), agent.py:281-341
  * (RecurrentModel), agent.py:1021-1051 (representation / transition).  C[M,N] = op(A) op(B) (+bias) (+C).
- * A is [M,K] (lda) or [K,M] if transA; B is [K,N] (ldb) or [N,K] if transB (nn.Linear weight layout). */
+ * A is [M,K] (lda) or [K,M] if transA; B is [K,N] (ldb) or [N,K] if transB (nn.Linear weight layout).  K = 0 gives
+ * C = bias (or 0), or C += bias when accumulating.  The FFMA routes (every tile config, split-K, the rank-K kernel, K = 0)
+ * are checked against a float64 reference (tests/test_gpu_simt_precision.py). */
 int b200rl_gemm_f32(const float* A, const float* B, float* C, const float* bias, int M, int N, int K, int lda, int ldb,
                     int ldc, int transA, int transB, int accumulate, cudaStream_t stream);
 /* Tensor-core path used by b200rl_gemm_f32 for large NT products (transA = 0, transB = 1, 16-byte aligned
@@ -86,6 +88,12 @@ int b200rl_conv_up(const float* small_, const float* W, float* big, const float*
                    int Cb, cudaStream_t stream);
 int b200rl_conv_wgrad(const float* small_, const float* big, float* dW, int NB, int h, int w, int Cs, int Cb,
                       int accumulate, cudaStream_t stream);
+/* Whether b200rl_conv_down / _up / _wgrad take their thin-channel kernels (conv_thin.cu: 1..4-channel big images, the
+ * RGB ends of the encoder / decoder) rather than the generic implicit GEMM.  These SIMT routes and the generic ones are
+ * checked against a float64 reference (tests/test_gpu_simt_precision.py). */
+int b200rl_thin_down_supported(int w, int Cs, int Cb);
+int b200rl_thin_up_supported(int Cs, int Cb);
+int b200rl_thin_wgrad_supported(int Cs, int Cb);
 /* Tensor-core implicit-GEMM versions of conv_down / conv_up (gemm_tc.cu: 4-D TMA boxes gather the taps, no
  * im2col buffer, 3xTF32 wgmma).  `Wpacked` is a caller-owned 16*Cs*Cb-float workspace filled by
  * b200rl_conv_pack (down: [Cs][tap][Cb]; up: [parity][Cb][tap][Cs]) after every weight update.  Eligible when the
@@ -251,7 +259,9 @@ int b200rl_gae(const float* rewards, const float* values, const float* dones, co
  * B(k,n) = B[k*sbk+n*sbn] (covers NN/NT/TN), C row-major with ldc.  epilogue: 0 none, 1 ReLU, 2 Tanh, 3 multiply by
  * ReLU'(aux), 4 multiply by Tanh'(aux) = 1-aux^2 (aux = the layer's saved activation output).  rsum (optional):
  * rsum[m] = sum_k A(m,k), i.e. the bias gradient when A = dY^T.  Replaces nn.Linear + activation forward/backward
- * of models/models.py:16-119 as used by sac/agent.py:19-108 and ppo/agent.py:84-177. */
+ * of models/models.py:16-119 as used by sac/agent.py:19-108 and ppo/agent.py:84-177.  Every tile config, epilogue and
+ * split-K form, up to the A2C weight gradients' K = 65536, is checked against a float64 reference
+ * (tests/test_gpu_simt_precision.py). */
 int b200rl_bgemm(const float* A, long long sam, long long sak, long long strideA, const float* B, long long sbk,
                  long long sbn, long long strideB, float* C, long long ldc, long long strideC, const float* bias,
                  long long strideBias, const float* aux, long long ldaux, long long strideAux, float* rsum,
@@ -327,7 +337,8 @@ int b200rl_lstm_seq_fwd(const float* xw, const float* W_hh, const float* h0, con
                         cudaStream_t stream);
 /* Backward through time in one launch: d_gates [T, B, 4H] = gradient w.r.t. the pre-activation gates from d_out
  * [T, B, H] and what the forward kept; zero at padded steps.  h0 / c0 get no gradient.  The weight, bias and input
- * gradients are dense products of d_gates done by the caller. */
+ * gradients are dense products of d_gates done by the caller.  Both kernels are checked against a float64 reference with
+ * propagated error bounds, for every sequences-per-CTA width (tests/test_gpu_simt_precision.py). */
 int b200rl_lstm_seq_bwd(const float* d_out, const float* W_hh, const float* gates, const float* cs, const float* c0,
                         const int* lengths, float* d_gates, int T, int B, int H, cudaStream_t stream);
 

@@ -543,9 +543,9 @@ extern "C" int b200rl_transpose2d(const float* X, float* Y, int rows, int cols, 
 }
 
 // thin-channel specialisations (conv_thin.cu)
-bool b200rl_thin_up_supported(int Cs, int Cb);
-bool b200rl_thin_wgrad_supported(int Cs, int Cb);
-bool b200rl_thin_down_supported(int w, int Cs, int Cb);
+extern "C" int b200rl_thin_up_supported(int Cs, int Cb);
+extern "C" int b200rl_thin_wgrad_supported(int Cs, int Cb);
+extern "C" int b200rl_thin_down_supported(int w, int Cs, int Cb);
 int b200rl_conv_down_thin(const float* big, const float* W, float* small, int NB, int h, int w, int Cs, int Cb, cudaStream_t st);
 int b200rl_conv_up_thin(const float* small, const float* W, float* big, const float* bias, int NB, int h, int w, int Cs,
                         int Cb, cudaStream_t st);

@@ -499,11 +499,11 @@ conv_wgrad_thin2_kernel(const float* __restrict__ small_, const float* __restric
 
 }  // namespace
 
-// internal entry points used by conv.cu's dispatchers
-bool b200rl_thin_up_supported(int Cs, int Cb) { return Cb == 3 && (Cs == 32 || Cs == 48 || Cs == 64 || Cs == 96); }
-bool b200rl_thin_wgrad_supported(int Cs, int Cb) { return Cb >= 1 && Cb <= 4 && Cs % 32 == 0 && Cs <= 128; }
+// dispatch predicates of conv.cu's b200rl_conv_{up,wgrad,down} (include/b200rl.h); the launchers below are internal
+extern "C" int b200rl_thin_up_supported(int Cs, int Cb) { return Cb == 3 && (Cs == 32 || Cs == 48 || Cs == 64 || Cs == 96); }
+extern "C" int b200rl_thin_wgrad_supported(int Cs, int Cb) { return Cb >= 1 && Cb <= 4 && Cs % 32 == 0 && Cs <= 128; }
 
-bool b200rl_thin_down_supported(int w, int Cs, int Cb) { return Cb == 3 && w == 32 && (Cs == 32 || Cs == 64 || Cs == 96); }
+extern "C" int b200rl_thin_down_supported(int w, int Cs, int Cb) { return Cb == 3 && w == 32 && (Cs == 32 || Cs == 64 || Cs == 96); }
 
 int b200rl_conv_down_thin(const float* big, const float* W, float* small, int NB, int h, int w, int Cs, int Cb, cudaStream_t st) {
   (void)w; (void)Cb;

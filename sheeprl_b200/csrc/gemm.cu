@@ -222,11 +222,14 @@ extern "C" int b200rl_gemm_f32(const float* A, const float* B, float* C, const f
   RL_CHECK_ARG(M >= 0 && N >= 0 && K >= 0, "negative dimension");
   if (M == 0 || N == 0) return B200RL_OK;
   RL_CHECK_ARG(lda >= (transA ? M : K) && ldb >= (transB ? K : N) && ldc >= N, "leading dimension too small");
-  if (K == 0) {
-    if (!accumulate) {
+  if (K == 0) {   // empty product: C = bias (or 0), or C += bias when accumulating
+    if (!accumulate)
       init2d_kernel<<<ceil_div((long long)M * N, 256), 256, 0, st>>>(C, bias, M, N, ldc);
-      RL_CHECK_LAUNCH();
-    }
+    else if (bias)
+      addbias2d_kernel<<<ceil_div((long long)M * N, 256), 256, 0, st>>>(C, bias, M, N, ldc);
+    else
+      return B200RL_OK;
+    RL_CHECK_LAUNCH();
     return B200RL_OK;
   }
   if (tc_enabled() && b200rl_gemm_tc_supported(A, B, M, N, K, lda, ldb, transA, transB))

@@ -120,7 +120,8 @@ __global__ void __launch_bounds__(256) bgemm_kernel(const BG g, const int ksplit
   const float* __restrict__ bias = g.bias ? g.bias + net * g.strideBias : nullptr;
   const float* __restrict__ aux = g.aux ? g.aux + net * g.strideAux : nullptr;
   if (ksplit > 1) {
-    // partial tile of a split-K product (plain epilogue, checked by the host): vector reductions where the row allows
+    // partial tile of a split-K product (plain epilogue, checked by the host): float2 reductions where the row allows.
+    // Only the 32x32 tile (TN = 2) is ever split: the host takes wider tiles only when they already fill the SMs.
 #pragma unroll
     for (int i = 0; i < TM; ++i) {
       const int m = m0 + ty * TM + i;
@@ -128,12 +129,7 @@ __global__ void __launch_bounds__(256) bgemm_kernel(const BG g, const int ksplit
       const int n = n0 + tx * TN;
       float* c = C + m * g.ldc + n;
       bool done = false;
-      if constexpr (TN == 4) {
-        if (n + 3 < g.N && ((reinterpret_cast<uintptr_t>(c) & 15) == 0)) {
-          atomicAdd(reinterpret_cast<float4*>(c), make_float4(acc[i][0], acc[i][1], acc[i][2], acc[i][3]));
-          done = true;
-        }
-      } else if constexpr (TN == 2) {
+      if constexpr (TN == 2) {
         if (n + 1 < g.N && ((reinterpret_cast<uintptr_t>(c) & 7) == 0)) {
           atomicAdd(reinterpret_cast<float2*>(c), make_float2(acc[i][0], acc[i][1]));
           done = true;
