@@ -150,8 +150,9 @@ int b200rl_kl_loss_grad(const float* post_mix, const float* prior_mix, float* d_
  * below are unused by the kernels; the fields stay so that the per-step path and this one fill the same set of saved
  * activations).  Requires B <= 16, S <= 64 categoricals of D <= 32 classes, even widths (R, Dx, Dr and S*D),
  * Dx <= 1024, R <= 1024 (at most two 4-column groups per CTA), Dr <= 4096 and the per-CTA weight slices to fit in
- * 227 KB of shared memory; the backward kernel needs more of it than the forward, so b200rl_rssm_scan_bwd_check can
- * refuse a model the forward runs.  Returns non-zero otherwise; the caller then uses the per-step ops.
+ * 227 KB of shared memory; the backward kernel needs more of it than the forward, so it can refuse a model the forward
+ * runs.  b200rl_rssm_scan_check answers that per direction; a caller asks it once and runs the per-step ops where it
+ * refuses.  The launches refuse the same models (and a short workspace) before launching anything.
  * Checked against a float64 reference (tests/test_gpu_rssm_scan.py) at widths up to R = Dx = 520 and Dx = 1024, one to
  * sixteen rows, S = 1 .. 64 and D = 1 .. 32. */
 typedef struct b200rl_rssm_scan_args {
@@ -186,8 +187,9 @@ int b200rl_rssm_scan_fwd(const b200rl_rssm_scan_args* args, cudaStream_t stream)
 /* BPTT over the same scan (autograd replay inside fabric.backward, dreamer_v3.py:191); must follow
  * b200rl_rssm_scan_fwd on the same workspace (uses its saved LayerNorm statistics and class indices). */
 int b200rl_rssm_scan_bwd(const b200rl_rssm_scan_args* args, const b200rl_rssm_scan_grads* grads, cudaStream_t stream);
-/* envelope check of the backward kernel for `args` (non-zero + last_error if it cannot run); launches nothing */
-int b200rl_rssm_scan_bwd_check(const b200rl_rssm_scan_args* args);
+/* envelope of the forward (backward = 0) or backward kernel for the dims of `args`: 0 if it runs them, non-zero +
+ * last_error if not.  Reads no pointer (the workspace included) and launches nothing. */
+int b200rl_rssm_scan_check(const b200rl_rssm_scan_args* args, int backward);
 int b200rl_rssm_scan_error(const void* workspace, cudaStream_t stream);
 /* cycle counters (2 x 32 int64: CTA 0, CTA 1) accumulated per phase by the last launch on `workspace` */
 int b200rl_rssm_scan_profile(const void* workspace, long long* out64, cudaStream_t stream);

@@ -85,7 +85,7 @@ class PlayerDV3:
         if mask is not None:
             raise NotImplementedError("action masks (MineDojo actor) are not built")
         e, ops, E = self.eng, self.eng.ops, self.num_envs
-        Z, R = e.Z, e.R
+        Z = e.Z
         if e.has_cnn:
             x = e.image_batch(obs, E)
             if x.dtype == torch.uint8:
@@ -112,13 +112,8 @@ class PlayerDV3:
                              e.g_pre, e.g_ln, self._h_next)
         self.recurrent_state[0].copy_(self._h_next)
         # posterior from [h, embed] (agent.py:451-465) and its sample
-        pr = "rssm.representation_model._model."
-        Wr1 = e._w(pr + "0.weight")
         e._project_embedding(e.rp_pre)
-        ops.gemm(self._h_next, Wr1[:, :R], e.rp_pre, False, True, accumulate=True)
-        ops.ln_act_fwd(e.rp_pre, e._w(pr + "1.weight"), e._w(pr + "1.bias"), e.eps, ACT_SILU, e.rp_act)
-        ops.gemm(e.rp_act, e._w(pr + "3.weight"), e.post_raw, False, True, bias=e._w(pr + "3.bias"))
-        ops.cat_sample(e.post_raw, nz, e.unimix, e.S, e.D, self.stochastic_state[0])
+        e._posterior_forward(self._h_next, e.rp_pre, e.rp_act, e.post_raw, nz, self.stochastic_state[0])
         # actor on [z, h] (agent.py:783-837)
         lat = e.latent                                                       # [E, Z+R] scratch row block
         ops.copy(self.stochastic_state[0], lat[:, :Z])

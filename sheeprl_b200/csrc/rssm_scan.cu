@@ -1333,7 +1333,13 @@ rssm_scan_bwd_kernel(const b200rl_rssm_scan_args a, const b200rl_rssm_scan_grads
 // the BASELINE S model runs the instantiation with compile-time widths
 bool fixed_dims(const b200rl_rssm_scan_args& a) { return a.S == 32 && a.D == 32 && a.R == 512 && a.Dx == 512 && a.Dr == 512; }
 
-int scan_check(const b200rl_rssm_scan_args& a) {
+size_t scan_smem(const b200rl_rssm_scan_args& a, bool backward) {
+  const Dims d{a.B, a.S, a.D, a.R, a.Dx, a.Dr, a.A};
+  return sizeof(float) * (size_t)(backward ? make_geo_b(d, 0).total : make_geo_f(d, 0).total);
+}
+
+// the envelope of one direction: dims and the shared-memory budget (the backward needs more of it than the forward)
+int scan_check(const b200rl_rssm_scan_args& a, bool backward) {
   RL_CHECK_ARG(a.B >= 1 && a.B <= MAXB, "persistent scan supports batch <= 16 rows per rank");
   RL_CHECK_ARG(a.D >= 1 && a.D <= 32, "persistent scan supports <= 32 classes per categorical");
   RL_CHECK_ARG(a.T >= 1 && a.S >= 1 && a.S <= 64, "persistent scan supports T >= 1 and 1 <= S <= 64 categoricals");
@@ -1343,6 +1349,11 @@ int scan_check(const b200rl_rssm_scan_args& a) {
   // one element of every per-step epilogue per thread (fixed assignments, rssm_scan.cu `Slot`)
   RL_CHECK_ARG(MAXB * owned_groups(a.R, 0) * 12 <= SCAN_NT, "persistent scan supports recurrent_state_size <= 1024");
   RL_CHECK_ARG(MAXB * owned_groups(a.Dr, 0) * 4 <= SCAN_NT, "persistent scan supports representation hidden_size <= 4096");
+  RL_CHECK_ARG(scan_smem(a, backward) <= 227 * 1024, "weight slices do not fit in shared memory for this model size");
+  return B200RL_OK;
+}
+
+int workspace_check(const b200rl_rssm_scan_args& a) {
   RL_CHECK_ARG(a.workspace && a.workspace_bytes >= (long long)ws_bytes(a.T, a.B, a.S, a.D, a.Dx, a.R, a.Dr), "workspace too small");
   return B200RL_OK;
 }
@@ -1356,10 +1367,9 @@ extern "C" long long b200rl_rssm_scan_workspace_bytes(int T, int B, int S, int D
 extern "C" int b200rl_rssm_scan_fwd(const b200rl_rssm_scan_args* args, cudaStream_t st) {
   RL_CHECK_ARG(args, "null args");
   const b200rl_rssm_scan_args& a = *args;
-  if (int rc = scan_check(a)) return rc;
-  const GeoF g = make_geo_f(Dims{a.B, a.S, a.D, a.R, a.Dx, a.Dr, a.A}, 0);
-  const size_t smem = sizeof(float) * (size_t)g.total;
-  RL_CHECK_ARG(smem <= 227 * 1024, "weight slices do not fit in shared memory for this model size");
+  if (int rc = scan_check(a, false)) return rc;
+  if (int rc = workspace_check(a)) return rc;
+  const size_t smem = scan_smem(a, false);
   const bool fix = fixed_dims(a);
   void* fn = fix ? (void*)rssm_scan_fwd_kernel<true> : (void*)rssm_scan_fwd_kernel<false>;
   RL_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1369,23 +1379,19 @@ extern "C" int b200rl_rssm_scan_fwd(const b200rl_rssm_scan_args* args, cudaStrea
   return B200RL_OK;
 }
 
-extern "C" int b200rl_rssm_scan_bwd_check(const b200rl_rssm_scan_args* args) {
+extern "C" int b200rl_rssm_scan_check(const b200rl_rssm_scan_args* args, int backward) {
   RL_CHECK_ARG(args, "null args");
-  if (int rc = scan_check(*args)) return rc;
-  const GeoB g = make_geo_b(Dims{args->B, args->S, args->D, args->R, args->Dx, args->Dr, args->A}, 0);
-  RL_CHECK_ARG(sizeof(float) * (size_t)g.total <= 227 * 1024, "weight slices do not fit in shared memory for this model size");
-  return B200RL_OK;
+  return scan_check(*args, backward != 0);
 }
 
 extern "C" int b200rl_rssm_scan_bwd(const b200rl_rssm_scan_args* args, const b200rl_rssm_scan_grads* grads,
                                     cudaStream_t st) {
   RL_CHECK_ARG(args && grads, "null args");
   const b200rl_rssm_scan_args& a = *args;
-  if (int rc = scan_check(a)) return rc;
+  if (int rc = scan_check(a, true)) return rc;
+  if (int rc = workspace_check(a)) return rc;
   RL_CHECK_ARG(grads->q_r && grads->q_g && grads->q_x, "q_r / q_g / q_x (pre-activation x weight products) are required");
-  const GeoB g = make_geo_b(Dims{a.B, a.S, a.D, a.R, a.Dx, a.Dr, a.A}, 0);
-  const size_t smem = sizeof(float) * (size_t)g.total;
-  RL_CHECK_ARG(smem <= 227 * 1024, "weight slices do not fit in shared memory for this model size");
+  const size_t smem = scan_smem(a, true);
   const bool fix = fixed_dims(a);
   void* fn = fix ? (void*)rssm_scan_bwd_kernel<true> : (void*)rssm_scan_bwd_kernel<false>;
   RL_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -22,7 +22,6 @@ Layouts (all fp32, row-major):
 from __future__ import annotations
 
 import math
-import os
 from typing import Dict, Mapping, Optional, Sequence
 
 import torch
@@ -149,7 +148,7 @@ def dense_ln_act(ops, x, W, gamma, beta, eps, act, out, pre=None, scratch=None):
     """out = act(LayerNorm(x W^T)) (the miniblock of sheeprl/utils/model.py:34-88, bias-free Linear).  Small row counts
     (imagination steps, heads on one batch) take the two-launch fused path of csrc/gemm_tc.cu; `pre` keeps x W^T for a
     backward and may be None there.  The unfused path needs somewhere to put x W^T: `pre`, else `scratch`."""
-    if (x.shape[0] <= FUSED_DENSE_MAX_ROWS and hasattr(ops, "gemm_ln_act") and ops.gemm_ln_supported(x, W)):
+    if x.shape[0] <= FUSED_DENSE_MAX_ROWS and ops.gemm_ln_supported(x, W):
         ops.gemm_ln_act(x, W, gamma, beta, eps, act, out, pre)
         return
     tmp = pre if pre is not None else scratch
@@ -453,13 +452,13 @@ class DV3Engine:
         if prec is not None and hasattr(self.ops, "set_matmul_precision"):
             self.ops.set_matmul_precision(str(prec))
         self._graph = None
-        # persistent fused RSSM scan (csrc/rssm_scan.cu) when the ops backend provides it and the shape qualifies
-        self.fused_scan = bool(hasattr(self.ops, "rssm_scan_fwd") and self.B <= 16 and self.D <= 32 and self.S <= 64)
+        # persistent fused RSSM scan (csrc/rssm_scan.cu) when the ops backend has it and the model is inside the kernels'
+        # envelope; the backward kernel needs more shared memory than the forward, so it can be refused alone
+        has_scan, dims = hasattr(self.ops, "rssm_scan_fwd"), self._scan_dims()
+        self.fused_scan = has_scan and self.ops.rssm_scan_supported(dims, backward=False)
+        self.fused_scan_bwd = has_scan and self.ops.rssm_scan_supported(dims, backward=True)
         self._scan_ws = None
         self._scan_q = None
-        self._scan_bwd_checked = False
-        self.fused_scan_bwd = hasattr(self.ops, "rssm_scan_bwd") and os.environ.get("B200RL_SCAN_BWD", "1") != "0"
-        self._fused_fwd_done = False
 
     # ------------------------------------------------------------------ CUDA-graph replay of the step
     def optimizer_groups(self):
@@ -772,8 +771,7 @@ class DV3Engine:
         ops, Z, R = self.ops, self.Z, self.R
         p = "rssm.recurrent_model."
         Win = self._w(p + "mlp._model.0.weight")
-        fused_x = (win_t is not None and hasattr(ops, "onehot_linear_ln")
-                   and ops.onehot_linear_ln_supported(win_t, x_act, x_pre if keep else None))
+        fused_x = win_t is not None and ops.onehot_linear_ln_supported(win_t, x_act, x_pre if keep else None)
         if fused_x:
             ops.onehot_linear_ln(z, act, win_t, self._w(p + "mlp._model.1.weight"), self._w(p + "mlp._model.1.bias"),
                                  self.eps, x_act, self.S, self.D, pre=x_pre if keep else None)
@@ -786,8 +784,7 @@ class DV3Engine:
             ops.ln_act_fwd(x_pre, self._w(p + "mlp._model.1.weight"), self._w(p + "mlp._model.1.bias"), self.eps,
                            ACT_SILU, x_act)
         Wg = self._w(p + "rnn.linear.weight")
-        if (hx is not None and hx.shape[0] <= FUSED_DENSE_MAX_ROWS and hasattr(ops, "gemm_ln_gru")
-                and ops.gemm_ln_supported(hx, Wg, 1)):
+        if hx is not None and hx.shape[0] <= FUSED_DENSE_MAX_ROWS and ops.gemm_ln_supported(hx, Wg, 1):
             # product + split-K sum + LayerNorm + gate in two launches; the new h also lands in `h_next` (the next
             # step's [h | x] input)
             ops.gemm_ln_gru(hx, Wg, self._w(p + "rnn.layer_norm.weight"), self._w(p + "rnn.layer_norm.bias"), self.eps,
@@ -803,6 +800,25 @@ class DV3Engine:
         ops.gru_gate_fwd(g_ln, h_prev, h_out)
         return False
 
+    def _recurrent_backward(self, g_ln, h_prev, g_pre, x_pre, dh, d_g_ln, d_g_pre, d_x_act, d_x_pre, dh_prev, dz,
+                            da=None):
+        """Data-gradient backward of `_recurrent_forward` (its parameter gradients are batched products of the caller):
+        dh, the gradient of the new h -> dh_prev (gradient of h_prev) and dz (of z); `da`: also the gradient of the
+        action columns."""
+        ops, Z, R = self.ops, self.Z, self.R
+        p = "rssm.recurrent_model."
+        Win, Wg = self._w(p + "mlp._model.0.weight"), self._w(p + "rnn.linear.weight")
+        ops.gru_gate_bwd(g_ln, h_prev, dh, d_g_ln, dh_prev)
+        ops.ln_act_bwd(g_pre, self._w(p + "rnn.layer_norm.weight"), self._w(p + "rnn.layer_norm.bias"), self.eps, ACT_NONE,
+                       d_g_ln, d_g_pre, None, None)
+        ops.gemm(d_g_pre, Wg[:, :R], dh_prev, False, False, accumulate=True)
+        ops.gemm(d_g_pre, Wg[:, R:], d_x_act, False, False)
+        ops.ln_act_bwd(x_pre, self._w(p + "mlp._model.1.weight"), self._w(p + "mlp._model.1.bias"), self.eps, ACT_SILU,
+                       d_x_act, d_x_pre, None, None)
+        ops.gemm(d_x_pre, Win[:, :Z], dz, False, False)
+        if da is not None:
+            ops.gemm(d_x_pre, Win[:, Z:], da, False, False)
+
     def _transition_forward(self, h, tr_pre, tr_act, raw, keep: bool = True):
         ops = self.ops
         p = "rssm.transition_model._model."
@@ -810,18 +826,39 @@ class DV3Engine:
                      tr_act, tr_pre if keep else None, scratch=tr_pre)
         ops.gemm(tr_act, self._w(p + "3.weight"), raw, False, True, bias=self._w(p + "3.bias"))
 
+    def _transition_backward(self, raw, tr_pre, dz, dmix, d_raw, d_tr_act, d_tr_pre, dh, ln_grads: bool = False):
+        """Backward of `_transition_forward` and the categorical sample of its logits `raw`: the straight-through `dz`
+        and / or the unimix log-probabilities' `dmix` -> d_raw -> dh += gradient of h.  `ln_grads`: also write the
+        LayerNorm parameter gradients (the products' weight gradients are the caller's)."""
+        ops = self.ops
+        p = "rssm.transition_model._model."
+        ops.cat_sample_bwd(raw, dz, dmix, self.unimix, self.S, self.D, d_raw)
+        ops.gemm(d_raw, self._w(p + "3.weight"), d_tr_act, False, False)
+        ops.ln_act_bwd(tr_pre, self._w(p + "1.weight"), self._w(p + "1.bias"), self.eps, ACT_SILU, d_tr_act, d_tr_pre,
+                       self._gw(p + "1.weight") if ln_grads else None, self._gw(p + "1.bias") if ln_grads else None)
+        ops.gemm(d_tr_pre, self._w(p + "0.weight"), dh, False, False, accumulate=True)
+
+    def _posterior_forward(self, h, rp_pre, rp_act, raw, noise, z_out, mix_out=None):
+        """Representation model on [h | embed] and its sample z_out (agent.py:451-465).  `rp_pre` holds the embedding's
+        share of the first product on entry (`_project_embedding`); h's share is added to it."""
+        ops, R = self.ops, self.R
+        pr = "rssm.representation_model._model."
+        ops.gemm(h, self._w(pr + "0.weight")[:, :R], rp_pre, False, True, accumulate=True)
+        ops.ln_act_fwd(rp_pre, self._w(pr + "1.weight"), self._w(pr + "1.bias"), self.eps, ACT_SILU, rp_act)
+        ops.gemm(rp_act, self._w(pr + "3.weight"), raw, False, True, bias=self._w(pr + "3.bias"))
+        ops.cat_sample(raw, noise, self.unimix, self.S, self.D, z_out, mix_out)
+
     def _scan_forward(self, first: torch.Tensor):
-        """64-step RSSM scan (dreamer_v3.py:131-145, agent.py:396-435)."""
+        """64-step RSSM scan (dreamer_v3.py:131-145, agent.py:396-435): the posterior recurrence, then the prior of
+        every step off the recurrence."""
         ops, B, Z, R = self.ops, self.B, self.Z, self.R
         # learned initial state, identical for every row and step (agent.py:391-394)
         ops.tanh_fwd(self._w("rssm.initial_recurrent_state").view(1, R), self.h0)
         self._transition_forward(self.h0, self.init_tr_pre, self.init_tr_act, self.init_raw)
         ops.cat_sample(self.init_raw, None, self.unimix, self.S, self.D, self.z0)
-        pr = "rssm.representation_model._model."
-        Wr1 = self._w(pr + "0.weight")
-        if self.fused_scan and self._scan_forward_fused(first):
-            return
-        for t in range(self.T):
+        if self.fused_scan:
+            self._scan_forward_fused(first)
+        for t in (() if self.fused_scan else range(self.T)):
             s = slice(t * B, (t + 1) * B)
             f = first[s]
             if t == 0:
@@ -835,17 +872,10 @@ class DV3Engine:
             h = self.latent[s, Z:]
             self._recurrent_forward(self.z_in[s], self.a_in[s], self.h_in[s], self.x_pre[s], self.x_act[s],
                                     self.g_pre[s], self.g_ln[s], h)
-            self._transition_forward(h, self.tr_pre[s], self.tr_act[s], self.prior_raw[s])
-            # prior: only its unimix log-probs are needed (the prior sample is discarded, dreamer_v3.py:135)
-            ops.cat_sample(self.prior_raw[s], None, self.unimix, self.S, self.D, None, self.prior_mix[s])
             ops.copy(self.pe[s], self.rp_pre[s])
-            ops.gemm(h, Wr1[:, :R], self.rp_pre[s], False, True, accumulate=True)
-            ops.ln_act_fwd(self.rp_pre[s], self._w(pr + "1.weight"), self._w(pr + "1.bias"), self.eps, ACT_SILU,
-                           self.rp_act[s])
-            ops.gemm(self.rp_act[s], self._w(pr + "3.weight"), self.post_raw[s], False, True,
-                     bias=self._w(pr + "3.bias"))
-            ops.cat_sample(self.post_raw[s], self.noise_post[t], self.unimix, self.S, self.D, self.latent[s, :Z],
-                           self.post_mix[s])
+            self._posterior_forward(h, self.rp_pre[s], self.rp_act[s], self.post_raw[s], self.noise_post[t],
+                                    self.latent[s, :Z], self.post_mix[s])
+        self._prior_forward()
 
     def _prior_forward(self):
         """The prior of every step (transition model on h_t, agent.py:433) is off the recurrence: with the h sequence
@@ -855,24 +885,12 @@ class DV3Engine:
         # only the prior's unimix log-probs are needed (the prior sample is discarded, dreamer_v3.py:135)
         self.ops.cat_sample(self.prior_raw, None, self.unimix, self.S, self.D, None, self.prior_mix)
 
-    def _scan_forward_fused(self, first: torch.Tensor) -> bool:
-        """The posterior recurrence of the scan as ONE persistent cooperative kernel (csrc/rssm_scan.cu), the prior
-        batched behind it.  Produces exactly the saved activations of the per-step path above.  Returns False (and
-        disables itself) if the model does not fit the kernel's shared-memory budget."""
+    def _scan_forward_fused(self, first: torch.Tensor):
+        """The posterior recurrence of the scan as ONE persistent cooperative kernel (csrc/rssm_scan.cu).  Produces
+        exactly the saved activations of the per-step path."""
         if self._scan_ws is None:
             self._scan_ws = self.ops.rssm_scan_workspace(self.T, self.B, self.S, self.D, self.Dx, self.R, self.Dr)
-        tensors = self._scan_tensors(first)
-        dims = self._scan_dims()
-        try:
-            self.ops.rssm_scan_fwd(dims, self.eps, self.unimix, tensors, self._scan_ws)
-        except Exception as e:  # shape outside the kernel's envelope: keep the per-step kernels
-            if "shared memory" in str(e) or "supports" in str(e):
-                self.fused_scan = False
-                return False
-            raise
-        self._prior_forward()
-        self._fused_fwd_done = True
-        return True
+        self.ops.rssm_scan_fwd(self._scan_dims(), self.eps, self.unimix, self._scan_tensors(first), self._scan_ws)
 
     def _scan_dims(self):
         return dict(T=self.T, B=self.B, S=self.S, D=self.D, R=self.R, A=self.A, Dx=self.Dx, Dt=self.Dt, Dr=self.Dr,
@@ -895,21 +913,16 @@ class DV3Engine:
 
     def _prior_backward(self):
         """Backward of the batched prior: its gradient comes from the KL term only (d_prior_mix), so it does not depend on
-        the BPTT either; its contribution to dh is added to d_latent before the backward scan starts.  Also writes the
+        the BPTT; its contribution to dh is added to d_latent before the backward scan starts.  Also writes the
         transition model's LayerNorm parameter gradients."""
-        ops, Z = self.ops, self.Z
-        pt = "rssm.transition_model._model."
-        ops.cat_sample_bwd(self.prior_raw, None, self.d_prior_mix, self.unimix, self.S, self.D, self.d_prior_raw)
-        ops.gemm(self.d_prior_raw, self._w(pt + "3.weight"), self.d_tr_act, False, False)
-        ops.ln_act_bwd(self.tr_pre, self._w(pt + "1.weight"), self._w(pt + "1.bias"), self.eps, ACT_SILU,
-                       self.d_tr_act, self.d_tr_pre, self._gw(pt + "1.weight"), self._gw(pt + "1.bias"))
-        ops.gemm(self.d_tr_pre, self._w(pt + "0.weight"), self.d_latent[:, Z:], False, False, accumulate=True)
+        self._transition_backward(self.prior_raw, self.tr_pre, None, self.d_prior_mix, self.d_prior_raw, self.d_tr_act,
+                                  self.d_tr_pre, self.d_latent[:, self.Z:], ln_grads=True)
 
-    def _scan_backward_fused(self, first: torch.Tensor) -> bool:
-        """BPTT of the posterior recurrence as ONE persistent cooperative kernel.  Before it: the batched prior backward
-        and the three `pre-activation x weight` products that let the kernel apply every LayerNorm-backward correction on
-        the consumer side (csrc/rssm_scan.cu).  It fills d_post_raw and the activation gradients d_rp_act / d_g_ln /
-        d_x_act; the deferred section turns those into the pre-activation gradients for all T*B rows at once."""
+    def _scan_backward_fused(self, first: torch.Tensor):
+        """BPTT of the posterior recurrence as ONE persistent cooperative kernel, after the three `pre-activation x
+        weight` products that let the kernel apply every LayerNorm-backward correction on the consumer side
+        (csrc/rssm_scan.cu).  It fills d_post_raw and the activation gradients d_rp_act / d_g_ln / d_x_act; the deferred
+        section turns those into the pre-activation gradients for all T*B rows at once."""
         ops, Z, R = self.ops, self.Z, self.R
         if self._scan_q is None:
             new = lambda *shape: torch.zeros(*shape, dtype=torch.float32, device=self.device)  # noqa: E731
@@ -920,37 +933,26 @@ class DV3Engine:
                      d_rp_pre=self.d_rp_pre, d_tr_act=self.d_tr_act, d_tr_pre=self.d_tr_pre, d_g_ln=self.d_g_ln,
                      d_g_pre=self.d_g_pre, d_x_act=self.d_x_act, d_x_pre=self.d_x_pre, d_h0=self.d_h0,
                      q_r=q_r, q_g=q_g, q_x=q_x)
-        tensors, dims = self._scan_tensors(first), self._scan_dims()
-        if not self._scan_bwd_checked:          # envelope check before anything is launched (first call only)
-            try:
-                ops.rssm_scan_bwd_check(dims, self.eps, self.unimix, tensors, grads, self._scan_ws)
-            except Exception as e:
-                if "shared memory" in str(e) or "supports" in str(e):
-                    self.fused_scan_bwd = False
-                    return False
-                raise
-            self._scan_bwd_checked = True
-        self._prior_backward()
         p, pr = "rssm.recurrent_model.", "rssm.representation_model._model."
         ops.gemm(self.rp_pre, self._w(pr + "0.weight")[:, :R], q_r, False, False)
         ops.gemm(self.g_pre, self._w(p + "rnn.linear.weight"), q_g, False, False)
         ops.gemm(self.x_pre, self._w(p + "mlp._model.0.weight")[:, :Z], q_x, False, False)
-        ops.rssm_scan_bwd(dims, self.eps, self.unimix, tensors, grads, self._scan_ws)
-        return True
+        ops.rssm_scan_bwd(self._scan_dims(), self.eps, self.unimix, self._scan_tensors(first), grads, self._scan_ws)
 
     def _scan_backward(self, first: torch.Tensor):
-        """BPTT over the scan (SURVEY.md App. E).  Per-step only the data-gradient GEMMs run; the weight
-        gradients are single big GEMMs over all T*B rows afterwards."""
+        """BPTT over the scan (SURVEY.md App. E): the batched prior backward, then the posterior recurrence.  Per step
+        only the data-gradient GEMMs run; the weight gradients are single big GEMMs over all T*B rows afterwards."""
         ops, B, Z, R = self.ops, self.B, self.Z, self.R
         p = "rssm.recurrent_model."
         pt, pr = "rssm.transition_model._model.", "rssm.representation_model._model."
-        Win, Wg = self._w(p + "mlp._model.0.weight"), self._w(p + "rnn.linear.weight")
         Wr1 = self._w(pr + "0.weight")
         ops.zero(self.dz_carry)
         ops.zero(self.dh_carry)
         ops.zero(self.d_h0)
-        fused = self.fused_scan and self.fused_scan_bwd and self._fused_fwd_done and self._scan_backward_fused(first)
-        self._fused_fwd_done = False
+        self._prior_backward()
+        fused = self.fused_scan and self.fused_scan_bwd
+        if fused:
+            self._scan_backward_fused(first)
         for t in (() if fused else reversed(range(self.T))):
             s = slice(t * B, (t + 1) * B)
             f = first[s]
@@ -965,22 +967,9 @@ class DV3Engine:
             ops.ln_act_bwd(self.rp_pre[s], self._w(pr + "1.weight"), self._w(pr + "1.bias"), self.eps, ACT_SILU,
                            self.d_rp_act[s], self.d_rp_pre[s], None, None)
             ops.gemm(self.d_rp_pre[s], Wr1[:, :R], self.dh_tot, False, False, accumulate=True)
-            # prior: KL only
-            ops.cat_sample_bwd(self.prior_raw[s], None, self.d_prior_mix[s], self.unimix, self.S, self.D,
-                               self.d_prior_raw[s])
-            ops.gemm(self.d_prior_raw[s], self._w(pt + "3.weight"), self.d_tr_act[s], False, False)
-            ops.ln_act_bwd(self.tr_pre[s], self._w(pt + "1.weight"), self._w(pt + "1.bias"), self.eps, ACT_SILU,
-                           self.d_tr_act[s], self.d_tr_pre[s], None, None)
-            ops.gemm(self.d_tr_pre[s], self._w(pt + "0.weight"), self.dh_tot, False, False, accumulate=True)
-            # GRU
-            ops.gru_gate_bwd(self.g_ln[s], self.h_in[s], self.dh_tot, self.d_g_ln[s], self.dh_in)
-            ops.ln_act_bwd(self.g_pre[s], self._w(p + "rnn.layer_norm.weight"), self._w(p + "rnn.layer_norm.bias"),
-                           self.eps, ACT_NONE, self.d_g_ln[s], self.d_g_pre[s], None, None)
-            ops.gemm(self.d_g_pre[s], Wg[:, :R], self.dh_in, False, False, accumulate=True)
-            ops.gemm(self.d_g_pre[s], Wg[:, R:], self.d_x_act[s], False, False)
-            ops.ln_act_bwd(self.x_pre[s], self._w(p + "mlp._model.1.weight"), self._w(p + "mlp._model.1.bias"),
-                           self.eps, ACT_SILU, self.d_x_act[s], self.d_x_pre[s], None, None)
-            ops.gemm(self.d_x_pre[s], Win[:, :Z], self.dz_in, False, False)
+            self._recurrent_backward(self.g_ln[s], self.h_in[s], self.g_pre[s], self.x_pre[s], self.dh_tot,
+                                     self.d_g_ln[s], self.d_g_pre[s], self.d_x_act[s], self.d_x_pre[s], self.dh_in,
+                                     self.dz_in)
             ops.mask_bwd(self.dz_in, f, self.dz_carry, None)
             ops.mask_bwd(self.dh_in, f, self.dh_carry, self.d_h0)
         # ---- deferred parameter gradients over all N rows
@@ -1006,9 +995,6 @@ class DV3Engine:
         # transition model
         ops.gemm(self.d_prior_raw, self.tr_act, gW(pt + "3.weight"), True, False)
         ops.col_sum(self.d_prior_raw, gW(pt + "3.bias"))
-        if not fused:                              # (the fused path's batched prior backward already did this one)
-            ops.ln_act_bwd(self.tr_pre, self._w(pt + "1.weight"), self._w(pt + "1.bias"), self.eps, ACT_SILU,
-                           self.d_tr_act, self.d_tr_pre, gW(pt + "1.weight"), gW(pt + "1.bias"))
         ops.gemm(self.d_tr_pre, h_all, gW(pt + "0.weight"), True, False)
         # recurrent model
         ops.ln_act_bwd(self.g_pre, self._w(p + "rnn.layer_norm.weight"), self._w(p + "rnn.layer_norm.bias"),
@@ -1072,7 +1058,7 @@ class DV3Engine:
         am = actor_mlp or self.actor_mlp
         # imagined z is an exact one-hot sample: its Linear is a gather over the transposed weight (refreshed here,
         # after the world-model update)
-        gather = hasattr(ops, "onehot_linear") and self.S <= 64 and self.A <= 32
+        gather = self.S <= 64 and self.A <= 32
         if gather:
             Win = self._w("rssm.recurrent_model.mlp._model.0.weight")
             if getattr(self, "_win_t", None) is None:
@@ -1110,7 +1096,7 @@ class DV3Engine:
                              actor.views[f"model._model.{3 * l + 1}.bias"], self.eps, ACT_SILU, am.act[l][rows],
                              am.pre[l][rows])
                 cur_in = am.act[l][rows]
-            if not self.is_continuous and hasattr(ops, "head_sample"):
+            if not self.is_continuous:
                 off, done = 0, True
                 for k, ad in enumerate(self.actions_dim):
                     Wh = actor.views[f"mlp_heads.{k}.weight"]
@@ -1146,12 +1132,10 @@ class DV3Engine:
         critic).  r_logits: the reward head's logits when that critic's reward is the task reward, None when it is a
         constant of the loss (the intrinsic reward).  rows[m] = discount * (advantage + entropy bonus / share); the
         bonus is counted in the first critic's rows only, its gradient once in the rollout backward."""
-        ops, N, H, Z, R, L, A = self.ops, self.N, self.H, self.Z, self.R, self.L, self.A
+        ops, N, H, Z, R, L = self.ops, self.N, self.H, self.Z, self.R, self.L
         a = self.cfg.algo
         ac = a.actor
         M1, M0 = (H + 1) * N, H * N
-        p = "rssm.recurrent_model."
-        pt = "rssm.transition_model._model."
         traj2, d_traj2 = self.traj.view(M1, L), self.d_traj.view(M1, L)
         for j, (mlp, v_logits, values, lam, moments, share, r_logits, rows) in enumerate(critics):
             ops.lambda_returns_bwd(c_logit.view(H + 1, N), self.discount, moments, lam, values, self.act_ent,
@@ -1163,7 +1147,6 @@ class DV3Engine:
             mlp.backward(traj2, self.d_v_logits, d_traj2, j > 0, data_only=True)
             if r_logits is not None:
                 self.rew_img.backward(traj2, self.d_r_logits, d_traj2, True, data_only=True)
-        Win, Wg = self._w(p + "mlp._model.0.weight"), self._w(p + "rnn.linear.weight")
         args = (float(ac.min_std), float(ac.max_std), float(ac.init_std), float(ac.action_clip))
         ops.zero(self.cd_dz_carry)
         ops.zero(self.cd_dh_carry)
@@ -1175,21 +1158,12 @@ class DV3Engine:
             ops.copy(self.d_traj[i][:, Z:], self.cd_dh)
             ops.axpy(self.cd_dh_carry, self.cd_dh)
             # z_i = straight-through sample of prior(h_i) -> transition MLP -> h_i
-            ops.cat_sample_bwd(self.c_raw[j], self.cd_dz, None, self.unimix, self.S, self.D, self.cd_raw)
-            ops.gemm(self.cd_raw, self._w(pt + "3.weight"), self.cd_tr_act, False, False)
-            ops.ln_act_bwd(self.c_tr_pre[j], self._w(pt + "1.weight"), self._w(pt + "1.bias"), self.eps, ACT_SILU,
-                           self.cd_tr_act, self.cd_tr_pre, None, None)
-            ops.gemm(self.cd_tr_pre, self._w(pt + "0.weight"), self.cd_dh, False, False, accumulate=True)
+            self._transition_backward(self.c_raw[j], self.c_tr_pre[j], self.cd_dz, None, self.cd_raw, self.cd_tr_act,
+                                      self.cd_tr_pre, self.cd_dh)
             # h_i = GRU(h_{i-1}, x_i), x_i = SiLU(LN(W_in [z_{i-1}, a_{i-1}]))
-            ops.gru_gate_bwd(self.c_g_ln[j], self.c_hx[j][:, :R], self.cd_dh, self.cd_g_ln, self.cd_dh_carry)
-            ops.ln_act_bwd(self.c_g_pre[j], self._w(p + "rnn.layer_norm.weight"), self._w(p + "rnn.layer_norm.bias"),
-                           self.eps, ACT_NONE, self.cd_g_ln, self.cd_g_pre, None, None)
-            ops.gemm(self.cd_g_pre, Wg[:, :R], self.cd_dh_carry, False, False, accumulate=True)
-            ops.gemm(self.cd_g_pre, Wg[:, R:], self.cd_x_act, False, False)
-            ops.ln_act_bwd(self.c_x_pre[j], self._w(p + "mlp._model.1.weight"), self._w(p + "mlp._model.1.bias"),
-                           self.eps, ACT_SILU, self.cd_x_act, self.cd_x_pre, None, None)
-            ops.gemm(self.cd_x_pre, Win[:, :Z], self.cd_dz_carry, False, False)
-            ops.gemm(self.cd_x_pre, Win[:, Z:], self.cd_a, False, False)
+            self._recurrent_backward(self.c_g_ln[j], self.c_hx[j][:, :R], self.c_g_pre[j], self.c_x_pre[j], self.cd_dh,
+                                     self.cd_g_ln, self.cd_g_pre, self.cd_x_act, self.cd_x_pre, self.cd_dh_carry,
+                                     self.cd_dz_carry, da=self.cd_a)
             # a_{i-1}: through the clipped rsample into the actor head; entropy bonus of step i-1
             rows = slice(j * N, (j + 1) * N)
             ops.cont_action_bwd(self.actor_raw[rows], self.noise_img_action[j], self.cd_a, self.discount[j],

@@ -478,10 +478,15 @@ class CudaOps:
                                                           c_int(Dr)))
         return torch.zeros((n + 3) // 4, dtype=torch.int32, device=self.device)
 
-    def _scan_args(self, dims: dict, eps: float, unimix: float, tensors: dict, workspace: torch.Tensor):
+    @staticmethod
+    def _scan_dims(dims: dict) -> RssmScanArgs:
         a = RssmScanArgs()
         for k in ("T", "B", "S", "D", "R", "A", "Dx", "Dt", "Dr", "ld_lat", "ld_wr1"):
             setattr(a, k, int(dims[k]))
+        return a
+
+    def _scan_args(self, dims: dict, eps: float, unimix: float, tensors: dict, workspace: torch.Tensor):
+        a = self._scan_dims(dims)
         a.eps, a.unimix = float(eps), float(unimix)
         for name in RssmScanArgs.POINTERS:
             t = tensors[name]
@@ -497,13 +502,9 @@ class CudaOps:
         a = self._scan_args(dims, eps, unimix, tensors, workspace)
         self._ck(self.lib.b200rl_rssm_scan_fwd(ctypes.byref(a), self._st()))
 
-    def rssm_scan_bwd_check(self, dims: dict, eps: float, unimix: float, tensors: dict, grads: dict,
-                            workspace: torch.Tensor):
-        """raises if the model is outside the backward kernel's envelope; launches nothing"""
-        a = self._scan_args(dims, eps, unimix, tensors, workspace)
-        rc = self.lib.b200rl_rssm_scan_bwd_check(ctypes.byref(a))
-        if rc != 0:
-            raise B200RLError(self.lib.b200rl_last_error().decode())
+    def rssm_scan_supported(self, dims: dict, backward: bool) -> bool:
+        """whether the forward / backward kernel runs a model of these dims (`rssm_scan_fwd`'s keys); launches nothing"""
+        return self.lib.b200rl_rssm_scan_check(ctypes.byref(self._scan_dims(dims)), c_int(int(backward))) == 0
 
     def rssm_scan_bwd(self, dims: dict, eps: float, unimix: float, tensors: dict, grads: dict,
                       workspace: torch.Tensor):

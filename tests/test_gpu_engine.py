@@ -2,7 +2,6 @@
   * against the committed reference fixtures (tests/golden, produced by the unmodified reference train());
   * against the oracle on the BASELINE config (S, B=16, T=64, H=15), incl. gradients;
   * size-independent properties at full size (finite, deterministic replay, sample one-hotness)."""
-import os
 
 import pytest
 import torch
@@ -203,7 +202,7 @@ def test_fused_scan_equals_per_step_scan(name):
             if name == "mixed_bwd":
                 assert not eng.fused_scan_bwd, "the backward kernel should not fit this model"
             else:
-                assert eng.fused_scan_bwd or os.environ.get("B200RL_SCAN_BWD", "1") == "0", "fused backward scan was disabled"
+                assert eng.fused_scan_bwd, "fused backward scan was disabled"
             assert eng.ops.rssm_scan_error(eng._scan_ws) == 0, "a hand-off of the persistent scan timed out"
         outs.append({k: getattr(eng, k).clone() for k in (
             "latent", "z_in", "h_in", "a_in", "x_pre", "x_act", "g_pre", "g_ln", "tr_pre", "tr_act", "rp_pre", "rp_act",

@@ -149,6 +149,7 @@ def test_scan_kernels_match_float64_reference(ops, key, unimix):
     T, B, S, D, R, Dx, Dr, A = CASES[key]
     Z = S * D
     dims, t, gr = make_problem(CASES[key], seed=100 + list(CASES).index(key), zero_start=key in ZERO_START)
+    assert ops.rssm_scan_supported(dims, backward=False) and ops.rssm_scan_supported(dims, backward=True)
     ws = ops.rssm_scan_workspace(T, B, S, D, Dx, R, Dr)
     fwd = run_fwd(ops, dims, unimix, t, ws)
     pre_products(ops, dims, t, gr)
@@ -228,20 +229,23 @@ REFUSALS = {
 
 
 @pytest.mark.parametrize("name", list(REFUSALS))
-def test_scan_refuses_outside_envelope(ops, name):
-    """Every refusal happens before anything is launched (all outputs stay untouched).  The messages the engine can meet
-    contain "supports" or "shared memory": that is how it recognises a model to run on the per-step kernels."""
+def test_scan_check_and_launches_refuse_outside_envelope(ops, name):
+    """The envelope query refuses every model outside the envelope in both directions (the engine asks it once, at
+    construction, to choose between the persistent and the per-step kernels); the launches refuse the same models, and a
+    short workspace, before anything is launched (all outputs stay untouched)."""
     from sheeprl_b200.lib import B200RLError
 
     T, B, S, D, R, Dx, Dr, A = REFUSALS[name]
     dims, t, gr = make_problem(REFUSALS[name], seed=7)
     ws = ops.rssm_scan_workspace(T, B, S, D, Dx, R, Dr)
+    in_envelope = name == "short_workspace"           # the query reads dims only
+    assert ops.rssm_scan_supported(dims, backward=False) == in_envelope
+    assert ops.rssm_scan_supported(dims, backward=True) == in_envelope
     if name == "short_workspace":
         ws, match = ws[:-1], "workspace"
     else:
         match = "supports|shared memory"
     for call in (lambda: ops.rssm_scan_fwd(dims, EPS, 0.01, t, ws),
-                 lambda: ops.rssm_scan_bwd_check(dims, EPS, 0.01, t, gr, ws),
                  lambda: ops.rssm_scan_bwd(dims, EPS, 0.01, t, gr, ws)):
         with pytest.raises(B200RLError, match=match):
             call()
