@@ -99,7 +99,10 @@ int b200rl_thin_wgrad_supported(int Cs, int Cb);
  * b200rl_conv_pack (down: [Cs][tap][Cb]; up: [parity][Cb][tap][Cs]) after every weight update.  Eligible when the
  * gathered image has a multiple of 32 channels and the small grid tiles by 128 pixels (`_supported`). */
 /* Weight gradient as one tensor-core GEMM over all pixels: small^T [Cs][P] times the transposed im2col of `big`
- * [16*Cb][P] (both K-major, split-K).  `workspace`: b200rl_conv_wgrad_tc_workspace(...) floats, caller-owned. */
+ * [16*Cb][P] (both K-major, split-K).  `workspace`: b200rl_conv_wgrad_tc_workspace(...) floats, caller-owned.
+ * `_supported`: 1 for the shapes the launch runs, P = NB*h*w pixels in [1024, 2e9], Cs >= 48, Cb >= 8; b200rl_conv_wgrad
+ * runs every shape. */
+int b200rl_conv_wgrad_tc_supported(int NB, int h, int w, int Cs, int Cb);
 long long b200rl_conv_wgrad_tc_workspace(int NB, int h, int w, int Cs, int Cb);
 int b200rl_conv_wgrad_tc(const float* small_, const float* big, float* dW, float* workspace, int NB, int h, int w,
                          int Cs, int Cb, int accumulate, cudaStream_t stream);
@@ -131,7 +134,9 @@ int b200rl_cat_sample(const float* raw, const float* noise, float* onehot, float
                       cudaStream_t stream);
 /* Policy head + straight-through sample in one launch (Actor.mlp_heads[i] + OneHotCategoricalStraightThrough.rsample,
  * sheeprl/algos/dreamer_v3/agent.py:793-818): raw [M, A] = X W^T + bias, onehot = sample(unimix(raw), noise) with
- * b200rl_cat_sample's rule.  A <= 32, Kin <= 1024, Kin % 4 == 0, 16-byte aligned rows. */
+ * b200rl_cat_sample's rule.  A <= 32, Kin <= 1024, Kin % 4 == 0, 16-byte aligned rows: `_supported` is 1 for the
+ * operands the launch runs (it reads the pointer values, never through them). */
+int b200rl_head_sample_supported(const float* X, const float* W, int Kin, int A, long long ldx, long long ldw);
 int b200rl_head_sample(const float* X, const float* W, const float* bias, const float* noise, float* raw, float* onehot,
                        long long M, int Kin, int A, long long ldx, long long ldw, long long ldr, long long ldn,
                        long long ldo, float unimix, cudaStream_t stream);
@@ -346,12 +351,18 @@ int b200rl_lstm_seq_bwd(const float* d_out, const float* W_hh, const float* gate
 
 /* Linear([z, a]) for a one-hot z (S groups of K classes, straight-through categorical sample) as a gather-sum over the
  * transposed weight WT [S*K + A, N]: RecurrentModel.mlp's first Linear (agent.py:328-341) inside the imagination
- * rollout.  z: [M, S*K] (row stride ldz), act: [M, A], out: [M, N]. */
+ * rollout.  z: [M, S*K] (row stride ldz), act: [M, A], out: [M, N].  S <= 64 groups, A <= 32: `_supported` is 1 for
+ * the dims the launch runs. */
+int b200rl_onehot_linear_supported(int S, int K, int A, int N);
 int b200rl_onehot_linear(const float* z, const float* act, const float* WT, float* out, long long M, int S, int K, int A,
                          int N, long long ldz, long long lda, long long ldo, cudaStream_t stream);
 /* The same gather followed, in the same launch, by the miniblock's LayerNorm(eps) + SiLU: out = SiLU(LN(Linear([z, a])));
- * `pre` (optional) keeps the Linear output.  N a multiple of 128 up to 1024 (one float4 of the row per thread), 16-byte
- * aligned WT / gamma / beta / out / pre rows. */
+ * `pre` (optional) keeps the Linear output.  The dims of b200rl_onehot_linear_supported, N a multiple of 128 up to 1024
+ * (one float4 of the row per thread), 16-byte aligned WT / gamma / beta / out / pre rows.  `_ln_supported` answers the
+ * terms beyond b200rl_onehot_linear_supported's from the pointer values, without reading through them; a NULL pointer
+ * passes its alignment term (the launch refuses a NULL gamma or beta on its own). */
+int b200rl_onehot_linear_ln_supported(const float* WT, const float* gamma, const float* beta, const float* out,
+                                      const float* pre, int N, long long ldo, long long ldpre);
 int b200rl_onehot_linear_ln(const float* z, const float* act, const float* WT, const float* gamma, const float* beta,
                             float eps, float* pre, long long ldpre, float* out, long long M, int S, int K, int A, int N,
                             long long ldz, long long lda, long long ldo, cudaStream_t stream);

@@ -521,6 +521,9 @@ class EmulOps:
     def transpose2d(self, X: Tensor, Y: Tensor):
         Y.copy_(X.t())
 
+    def onehot_linear_supported(self, groups: int, classes: int, A: int, N: int) -> bool:
+        return groups <= 64 and A <= 32
+
     def onehot_linear(self, z: Tensor, act: Tensor, WT: Tensor, out: Tensor, groups: int, classes: int):
         Z = groups * classes
         out.copy_(z @ WT[:Z] + act @ WT[Z:])

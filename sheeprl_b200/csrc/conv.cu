@@ -497,11 +497,16 @@ extern "C" long long b200rl_conv_wgrad_tc_workspace(int NB, int h, int w, int Cs
 extern "C" int b200rl_conv_wgrad_mn(const float* small_, const float* big, float* G, int NB, int h, int w, int Cs, int Cb,
                                     cudaStream_t st);
 
+extern "C" int b200rl_conv_wgrad_tc_supported(int NB, int h, int w, int Cs, int Cb) {
+  const long long P = (long long)NB * h * w;
+  return P >= 1024 && P <= 2000000000LL && Cs >= 48 && Cb >= 8;
+}
+
 extern "C" int b200rl_conv_wgrad_tc(const float* small_, const float* big, float* dW, float* workspace, int NB, int h,
                                     int w, int Cs, int Cb, int accumulate, cudaStream_t st) {
   RL_CHECK_ARG(small_ && big && dW && workspace, "null pointer");
+  RL_CHECK_ARG(b200rl_conv_wgrad_tc_supported(NB, h, w, Cs, Cb), "shape not eligible for the tensor-core wgrad path");
   const long long P = (long long)NB * h * w, Pp = (P + 3) / 4 * 4;
-  RL_CHECK_ARG(P >= 1024 && Cs >= 48 && Cb >= 8 && P <= 2000000000LL, "shape not eligible for the tensor-core wgrad path");
   if (b200rl_conv_wgrad_mn_supported(NB, h, w, Cs, Cb)) {
     // operands read in place: the gathered big image and the small image are both MN-major tiles
     float* G = workspace;                      // [16*Cb][Cs]

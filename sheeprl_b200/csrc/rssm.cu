@@ -498,12 +498,16 @@ extern "C" int b200rl_cat_sample(const float* raw, const float* noise, float* on
   return B200RL_OK;
 }
 
+extern "C" int b200rl_head_sample_supported(const float* X, const float* W, int Kin, int A, long long ldx, long long ldw) {
+  return A > 0 && A <= 32 && Kin > 0 && Kin <= 1024 && Kin % 4 == 0 && ldx % 4 == 0 && ldw % 4 == 0 &&
+         ((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(W)) & 15) == 0;
+}
+
 extern "C" int b200rl_head_sample(const float* X, const float* W, const float* bias, const float* noise, float* raw,
                                   float* onehot, long long M, int Kin, int A, long long ldx, long long ldw, long long ldr,
                                   long long ldn, long long ldo, float unimix, cudaStream_t st) {
   RL_CHECK_ARG(X && W && raw && onehot, "null pointer");
-  RL_CHECK_ARG(A > 0 && A <= 32 && Kin > 0 && Kin <= 1024 && Kin % 4 == 0 && ldx % 4 == 0 && ldw % 4 == 0 &&
-                   ((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(W)) & 15) == 0,
+  RL_CHECK_ARG(b200rl_head_sample_supported(X, W, Kin, A, ldx, ldw),
                "head_sample: A <= 32, Kin <= 1024, 16-byte aligned rows");
   if (M <= 0) return B200RL_OK;
   head_sample_kernel<<<ceil_div(M * 32, 256), 256, 0, st>>>(X, W, bias, noise, raw, onehot, M, Kin, A, ldx, ldw, ldr, ldn, ldo,
@@ -537,10 +541,21 @@ extern "C" int b200rl_kl_loss_grad(const float* post_mix, const float* prior_mix
   return B200RL_OK;
 }
 
+extern "C" int b200rl_onehot_linear_supported(int S, int K, int A, int N) {
+  return S > 0 && S <= 64 && K > 0 && A >= 0 && A <= 32 && N > 0;
+}
+
+extern "C" int b200rl_onehot_linear_ln_supported(const float* WT, const float* gamma, const float* beta, const float* out,
+                                                 const float* pre, int N, long long ldo, long long ldpre) {
+  return N >= 128 && N <= 1024 && N % 128 == 0 && ldo % 4 == 0 && ldpre % 4 == 0 &&
+         ((reinterpret_cast<uintptr_t>(WT) | reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta) |
+           reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(pre)) & 15) == 0;
+}
+
 extern "C" int b200rl_onehot_linear(const float* z, const float* act, const float* WT, float* out, long long M, int S,
                                     int K, int A, int N, long long ldz, long long lda, long long ldo, cudaStream_t st) {
   RL_CHECK_ARG(z && act && WT && out, "null pointer");
-  RL_CHECK_ARG(S > 0 && S <= 64 && K > 0 && A >= 0 && A <= 32 && N > 0, "bad dims (S <= 64 groups, A <= 32)");
+  RL_CHECK_ARG(b200rl_onehot_linear_supported(S, K, A, N), "bad dims (S <= 64 groups, A <= 32)");
   if (M <= 0) return B200RL_OK;
   onehot_linear_kernel<<<(unsigned)M, 256, 0, st>>>(z, act, WT, out, S, K, A, N, ldz, lda, ldo, nullptr, nullptr, 0.f, nullptr, 0);
   RL_CHECK_LAUNCH();
@@ -552,11 +567,9 @@ extern "C" int b200rl_onehot_linear_ln(const float* z, const float* act, const f
                                        int S, int K, int A, int N, long long ldz, long long lda, long long ldo,
                                        cudaStream_t st) {
   RL_CHECK_ARG(z && act && WT && out && gamma && beta, "null pointer");
-  RL_CHECK_ARG(S > 0 && S <= 64 && K > 0 && A >= 0 && A <= 32 && N >= 128 && N <= 1024 && N % 128 == 0,
-               "bad dims (S <= 64 groups, A <= 32, N a multiple of 128 up to 1024)");
-  RL_CHECK_ARG(((reinterpret_cast<uintptr_t>(WT) | reinterpret_cast<uintptr_t>(gamma) | reinterpret_cast<uintptr_t>(beta) |
-                 reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(pre)) & 15) == 0 && ldo % 4 == 0 && ldpre % 4 == 0,
-               "onehot_linear_ln needs 16-byte aligned rows");
+  RL_CHECK_ARG(b200rl_onehot_linear_supported(S, K, A, N), "bad dims (S <= 64 groups, A <= 32)");
+  RL_CHECK_ARG(b200rl_onehot_linear_ln_supported(WT, gamma, beta, out, pre, N, ldo, ldpre),
+               "onehot_linear_ln: N a multiple of 128 up to 1024, 16-byte aligned rows");
   if (M <= 0) return B200RL_OK;
   onehot_linear_kernel<<<(unsigned)M, N / 4, 0, st>>>(z, act, WT, out, S, K, A, N, ldz, lda, ldo, gamma, beta, eps, pre, ldpre);
   RL_CHECK_LAUNCH();

@@ -1058,9 +1058,9 @@ class DV3Engine:
         am = actor_mlp or self.actor_mlp
         # imagined z is an exact one-hot sample: its Linear is a gather over the transposed weight (refreshed here,
         # after the world-model update)
-        gather = self.S <= 64 and self.A <= 32
+        Win = self._w("rssm.recurrent_model.mlp._model.0.weight")
+        gather = ops.onehot_linear_supported(self.S, self.D, self.A, Win.shape[0])
         if gather:
-            Win = self._w("rssm.recurrent_model.mlp._model.0.weight")
             if getattr(self, "_win_t", None) is None:
                 self._win_t = torch.empty(Win.shape[1], Win.shape[0], dtype=torch.float32, device=self.device)
             ops.transpose2d(Win, self._win_t)

@@ -6,6 +6,7 @@ import pytest
 import torch
 
 from oracle.ops_emul import EmulOps
+from tests.test_lib_cpu import HEAD_SAMPLE, ONEHOT_LINEAR, WGRAD_TC
 
 pytestmark = pytest.mark.gpu
 
@@ -721,3 +722,67 @@ def test_head_sample_equals_linear_then_cat_sample(ops, M, Kin, A, unimix):
     cu.cat_sample(raw_all[:, 3:], qg[:, 2:2 + A], unimix, 1, A, hot2)
     assert torch.equal(hot2, act_all[:, 3:])
     assert float(raw_all[:, :3].abs().max()) == 0.0 and float(act_all[:, :3].abs().max()) == 0.0
+
+
+def _nan(n, off=0):
+    """n NaN floats starting `off` floats into a fresh (16-byte aligned) allocation"""
+    return torch.full((n + off,), float("nan"), device="cuda")[off:]
+
+
+def _runs_iff(ok, launch, *guards):
+    """`launch` runs when its query accepted the shape; otherwise it raises before any kernel runs and every guard keeps
+    its NaNs"""
+    from sheeprl_b200.lib import B200RLError
+
+    if ok:
+        launch()
+    else:
+        with pytest.raises(B200RLError, match="bad argument"):
+            launch()
+    torch.cuda.synchronize()
+    for g in guards:
+        assert bool(g.isnan().all()) != ok
+
+
+@pytest.mark.parametrize("case", list(HEAD_SAMPLE))
+def test_head_sample_launch_accepts_what_its_query_accepts(ops, case):
+    cu, _ = ops
+    Kin, A, xo, wo, ok = HEAD_SAMPLE[case]
+    M = 8
+    X, W = _nan(M * Kin, xo).view(M, Kin).normal_(), _nan(A * Kin, wo).view(A, Kin).normal_()
+    raw, hot = _nan(M * A).view(M, A), _nan(M * A).view(M, A)
+    assert cu.head_sample_supported(X, W) == ok
+    _runs_iff(ok, lambda: cu.head_sample(X, W, None, None, 0.01, raw, hot), raw, hot)
+
+
+@pytest.mark.parametrize("case", list(ONEHOT_LINEAR))
+def test_onehot_linear_launches_accept_what_their_queries_accept(ops, case):
+    """the engine asks onehot_linear_supported, then onehot_linear_ln_supported for the fused form"""
+    cu, _ = ops
+    S, K, A, N, oo, gather, ln = ONEHOT_LINEAR[case]
+    M = 8
+    z = torch.nn.functional.one_hot(torch.randint(0, K, (M, S)), K).float().reshape(M, S * K).cuda()
+    act, WT = torch.randn(M, A, device="cuda"), 0.1 * torch.randn(S * K + A, N, device="cuda")
+    gamma, beta = torch.ones(N, device="cuda"), torch.zeros(N, device="cuda")
+    out, out_ln = _nan(M * N, oo).view(M, N), _nan(M * N, oo).view(M, N)
+    assert cu.onehot_linear_supported(S, K, A, N) == gather
+    assert (gather and cu.onehot_linear_ln_supported(WT, out_ln)) == ln
+    _runs_iff(gather, lambda: cu.onehot_linear(z, act, WT, out, S, K), out)
+    _runs_iff(ln, lambda: cu.onehot_linear_ln(z, act, WT, gamma, beta, 1e-3, out_ln, S, K), out_ln)
+
+
+@pytest.mark.parametrize("case", [c for c, (NB, h, w, *_, ok) in WGRAD_TC.items() if not ok or NB * h * w <= 1 << 20])
+def test_conv_wgrad_tc_launch_accepts_what_its_query_accepts(ops, case):
+    cu, _ = ops
+    NB, h, w, Cs, Cb, ok = WGRAD_TC[case]
+    assert cu.lib.b200rl_conv_wgrad_tc_supported(NB, h, w, Cs, Cb) == ok
+    if NB * h * w <= 1 << 20:
+        small, big = torch.randn(NB, h, w, Cs, device="cuda"), torch.randn(NB, 2 * h, 2 * w, Cb, device="cuda")
+        ws = torch.empty(cu.lib.b200rl_conv_wgrad_tc_workspace(NB, h, w, Cs, Cb), device="cuda")
+    else:                       # a refused pixel count beyond any buffer: the launch reads no operand before refusing
+        small = big = ws = _nan(16)
+    dW = _nan(Cs * Cb * 16)
+    rc = cu.lib.b200rl_conv_wgrad_tc(small.data_ptr(), big.data_ptr(), dW.data_ptr(), ws.data_ptr(), NB, h, w, Cs, Cb,
+                                     0, cu._st())
+    torch.cuda.synchronize()
+    assert (rc == 0) == ok and bool(dW.isnan().all()) != ok

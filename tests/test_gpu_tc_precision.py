@@ -55,8 +55,6 @@ def cu():
     ops = CudaOps("cuda")
     assert ops.use_tc, "the tensor-core paths are disabled (B200RL_DISABLE_TC=1)"
     assert ops.matmul_precision() == "highest"
-    ops.lib.b200rl_conv_wgrad_tc_workspace.restype = ctypes.c_longlong
-    ops.lib.b200rl_conv_pack_floats.restype = ctypes.c_longlong
     return ops
 
 
