@@ -230,6 +230,12 @@ int b200rl_sumsq(const float* x, long long n, double* out, cudaStream_t stream);
 int b200rl_adam_step(float* p, const float* g, float* m, float* v, const double* normsq, const int* step_dev,
                      float* norm_out, long long n, float max_norm, float lr, float b1, float b2, float eps,
                      cudaStream_t stream);
+/* adam_step with torch.optim.Adam's L2 weight decay (Dreamer-V2's optimizers, configs/algo/dreamer_v2.yaml:99,118,133):
+ * weight_decay * p is added to the clipped gradient before the moments.  weight_decay = 0 runs adam_step's kernel, bit
+ * for bit; weight_decay < 0 is refused.  Covered by tests/test_gpu_adam_wd.py. */
+int b200rl_adam_step_wd(float* p, const float* g, float* m, float* v, const double* normsq, const int* step_dev,
+                        float* norm_out, long long n, float max_norm, float lr, float b1, float b2, float eps,
+                        float weight_decay, cudaStream_t stream);
 /* fabric.clip_gradients + torch.optim.RMSprop.step (single-tensor path; A2C, a2c/a2c.py:102-105) in one pass, with
  * adam_step's normsq / norm_out contract.  square_avg always; momentum_buf read and written only when momentum > 0;
  * grad_avg non-NULL selects `centered`.  eps is added after the square root; the step count does not enter the update. */

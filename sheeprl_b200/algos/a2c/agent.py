@@ -36,7 +36,7 @@ def opt_from_cfg(cfg) -> dict:
                                   "torch.optim.RMSprop and torch.optim.Adam")
     if name == "Adam":
         return {"name": "adam", "lr": float(o.lr), "eps": float(o.get("eps", 1e-8)),
-                "betas": tuple(o.get("betas", (0.9, 0.999)))}
+                "betas": tuple(o.get("betas", (0.9, 0.999))), "weight_decay": float(o.get("weight_decay", 0) or 0)}
     return {"name": "rmsprop", "lr": float(o.lr), "alpha": float(o.get("alpha", 0.99)), "eps": float(o.get("eps", 1e-8)),
             "weight_decay": float(o.get("weight_decay", 0) or 0), "momentum": float(o.get("momentum", 0) or 0),
             "centered": bool(o.get("centered", False))}

@@ -87,7 +87,7 @@ class A2CEngine(PPOEngine):
         if o["name"] == "adam":
             b1, b2 = o["betas"]
             self.ops.adam_step(g.flat, g.grad, g.exp_avg, g.exp_avg_sq, self.normsq, clip, lr, b1, b2, o["eps"],
-                               g.step_t, self.norm_out)
+                               g.step_t, self.norm_out, **g.adam_kwargs(o.get("weight_decay", 0.0)))
             return
         # RMSprop state in the group's buffers: square_avg -> exp_avg_sq, momentum_buffer -> exp_avg
         momentum = float(o["momentum"])

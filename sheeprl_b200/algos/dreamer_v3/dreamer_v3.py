@@ -25,19 +25,25 @@ class B200Adam(torch.optim.Optimizer):
     """Handle standing where the reference passes a `torch.optim.Adam` (dreamer_v3.py:448-457).  The update
     itself is the fused clip+Adam kernel inside the engine; this object is a real `torch.optim.Optimizer` (schedulers
     such as the reference's `PolynomialLR`, ppo.py:236-238, attach to it and the engine reads `param_groups[0]["lr"]`
-    before every fused step) whose `state_dict()` has torch's layout, so reference checkpoints round-trip."""
+    before every fused step) whose `state_dict()` has torch's layout, so reference checkpoints round-trip.
+    `weight_decay` is torch's L2 term (Dreamer-V2's optimizers default to 1e-6), added to the clipped gradient."""
 
     def __init__(self, group, names: Sequence[str], lr: float, eps: float, betas=(0.9, 0.999), weight_decay=0.0):
-        if weight_decay:
-            raise NotImplementedError("weight_decay != 0 is not supported by the fused Adam kernel")
+        if not float(weight_decay) >= 0.0:
+            raise ValueError(f"Invalid weight_decay value: {weight_decay}")
         self.group, self.names = group, list(names)
         super().__init__([group.views[n] for n in self.names],
-                         dict(lr=float(lr), betas=tuple(betas), eps=float(eps), weight_decay=0, amsgrad=False))
+                         dict(lr=float(lr), betas=tuple(betas), eps=float(eps), weight_decay=float(weight_decay),
+                              amsgrad=False))
         group.optimizer = self
 
     @property
     def lr(self) -> float:
         return float(self.param_groups[0]["lr"])
+
+    @property
+    def weight_decay(self) -> float:
+        return float(self.param_groups[0]["weight_decay"])
 
     def zero_grad(self, set_to_none: bool = True):  # gradients live in the engine's flat buffer
         return None
@@ -82,7 +88,7 @@ class B200Adam(torch.optim.Optimizer):
         self.group.step = steps.pop() if steps else 0
         self.group.step_t.fill_(self.group.step)
         if sd.get("param_groups"):
-            for k in ("lr", "eps", "betas"):
+            for k in ("lr", "eps", "betas", "weight_decay"):
                 if k in sd["param_groups"][0]:
                     self.param_groups[0][k] = sd["param_groups"][0][k]
         eng = getattr(self, "rng_engine", None)

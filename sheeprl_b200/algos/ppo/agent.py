@@ -210,7 +210,8 @@ def build_agent(fabric, actions_dim: Sequence[int], is_continuous: bool, cfg: Di
         ops = CudaOps()
     spec = spec_from_cfg(cfg, actions_dim, is_continuous, obs_space)
     o = cfg.algo.optimizer
-    opt = {"lr": float(o.lr), "eps": float(o.eps), "betas": tuple(o.get("betas", (0.9, 0.999)))}
+    opt = {"lr": float(o.lr), "eps": float(o.eps), "betas": tuple(o.get("betas", (0.9, 0.999))),
+           "weight_decay": float(o.get("weight_decay", 0) or 0)}
     eng = PPOEngine(spec, hp_from_cfg(cfg), opt, fabric.device, ops, seed=int(cfg.get("seed", 0) or 0))
     g = torch.Generator().manual_seed(int(cfg.get("seed", 0) or 0))
     ortho = "feature_extractor." if cfg.algo.encoder.ortho_init else None

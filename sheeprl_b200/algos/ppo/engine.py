@@ -389,7 +389,8 @@ class PPOEngine:
         """the fused clip + optimizer update of the flat group (gradient norm already in self.normsq)"""
         g = self.group
         self.ops.adam_step(g.flat, g.grad, g.exp_avg, g.exp_avg_sq, self.normsq, float(self.hp["max_grad_norm"]), lr,
-                           self.opt["betas"][0], self.opt["betas"][1], self.opt["eps"], g.step_t, self.norm_out)
+                           self.opt["betas"][0], self.opt["betas"][1], self.opt["eps"], g.step_t, self.norm_out,
+                           **g.adam_kwargs(self.opt.get("weight_decay", 0.0)))
 
     def train(self, data: Dict[str, torch.Tensor], index_batches: Sequence[Sequence[int]], on_minibatch=None):
         for ib in index_batches:

@@ -127,7 +127,8 @@ def build_agent(fabric, cfg: Dict[str, Any], obs_space, action_space, agent_stat
         ops = CudaOps()
 
     def opt(o):
-        return {"lr": float(o.lr), "eps": float(o.eps), "betas": tuple(o.get("betas", (0.9, 0.999)))}
+        return {"lr": float(o.lr), "eps": float(o.eps), "betas": tuple(o.get("betas", (0.9, 0.999))),
+                "weight_decay": float(o.get("weight_decay", 0) or 0)}
 
     eng = SACEngine(obs_dim, act_dim, int(cfg.algo.actor.hidden_size), int(cfg.algo.critic.hidden_size),
                     int(cfg.algo.critic.n), int(cfg.algo.get("per_rank_batch_size", 256)), float(cfg.algo.gamma),

@@ -127,7 +127,8 @@ class SACEngine:
         handle = getattr(group, "optimizer", None)          # B200Adam built by main / make_optimizers (schedulers edit it)
         lr = handle.lr if handle is not None else opt["lr"]
         self.ops.adam_step(group.flat, group.grad, group.exp_avg, group.exp_avg_sq, self.zero_normsq, 0.0, lr,
-                           opt["betas"][0], opt["betas"][1], opt["eps"], group.step_t, self.norm_out)
+                           opt["betas"][0], opt["betas"][1], opt["eps"], group.step_t, self.norm_out,
+                           **group.adam_kwargs(opt.get("weight_decay", 0.0)))
 
     # ------------------------------------------------------------------ the update
     def train_step(self, data: Dict[str, torch.Tensor], do_ema: bool, noise: Optional[Dict[str, torch.Tensor]] = None):

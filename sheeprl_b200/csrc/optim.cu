@@ -1,7 +1,8 @@
 // Optimiser + small utility kernels on the flat parameter groups (pure HBM streaming).
 //
 // Replaces (reference): fabric.clip_gradients -> torch.nn.utils.clip_grad_norm_ and torch.optim.Adam.step
-// (dreamer_v3.py:191-200, :298-304, :318-327; configs/optim/adam.yaml), torch.optim.RMSprop.step (a2c/a2c.py:102-105;
+// (dreamer_v3.py:191-200, :298-304, :318-327; configs/optim/adam.yaml), torch.optim.Adam(weight_decay > 0).step
+// (dreamer_v2.py:202-209, :333-337, :349-356; configs/algo/dreamer_v2.yaml), torch.optim.RMSprop.step (a2c/a2c.py:102-105;
 // configs/optim/rmsprop.yaml), the per-parameter target-critic EMA
 // loop (dreamer_v3.py:674-680), torch.multinomial's Exp(1) noise (Philox4x32-10 here).
 // Clip + Adam are one pass: 4 reads + 3 writes of 4 B per parameter = 28 B/param (SURVEY.md §8d).
@@ -32,10 +33,13 @@ sumsq_kernel(const float* __restrict__ x, long long n, double* __restrict__ out)
   }
 }
 
+// WD: torch's L2 weight decay (torch/optim/adam.py: grad = grad.add(param, alpha=weight_decay)), added to the already
+// clipped gradient before the moments.  WD = false is the plain Adam kernel, so weight_decay = 0 stays bit-identical.
+template <bool WD>
 __global__ void __launch_bounds__(256)
 adam_step_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
                  const double* __restrict__ normsq, const int* __restrict__ step_t, float* __restrict__ norm_out,
-                 long long n, float max_norm, float lr, float b1, float b2, float eps, int vec) {
+                 long long n, float max_norm, float lr, float b1, float b2, float eps, float weight_decay, int vec) {
   __shared__ float s_coef, s_step_size, s_bc2_sqrt;
   if (threadIdx.x == 0) {
     const float total = (float)sqrt(*normsq);
@@ -56,6 +60,7 @@ adam_step_kernel(float* __restrict__ p, const float* __restrict__ g, float* __re
   const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   auto update = [&](float& pi, float gi, float& mi, float& vi) {
     gi *= coef;
+    if (WD) gi = gi + weight_decay * pi;
     mi = mi + omb1 * (gi - mi);            // exp_avg.lerp_(grad, 1 - beta1)
     vi = vi * b2 + omb2 * gi * gi;         // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value=1 - beta2)
     const float denom = sqrtf(vi) / bc2_sqrt + eps;
@@ -310,17 +315,25 @@ extern "C" int b200rl_sumsq(const float* x, long long n, double* out, cudaStream
   return B200RL_OK;
 }
 
-extern "C" int b200rl_adam_step(float* p, const float* g, float* m, float* v, const double* normsq, const int* step_t,
-                                float* norm_out, long long n, float max_norm, float lr, float b1, float b2, float eps,
-                                cudaStream_t st) {
+extern "C" int b200rl_adam_step_wd(float* p, const float* g, float* m, float* v, const double* normsq,
+                                   const int* step_t, float* norm_out, long long n, float max_norm, float lr, float b1,
+                                   float b2, float eps, float weight_decay, cudaStream_t st) {
   RL_CHECK_ARG(p && g && m && v && normsq && step_t && norm_out, "null pointer");
+  RL_CHECK_ARG(weight_decay >= 0.f, "weight_decay must be >= 0");
   if (n <= 0) return B200RL_OK;
   const int vec = ((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
                     reinterpret_cast<uintptr_t>(v)) & 15) == 0;
-  adam_step_kernel<<<stream_grid(vec ? (n + 3) / 4 : n), 256, 0, st>>>(p, g, m, v, normsq, step_t, norm_out, n, max_norm, lr,
-                                                                      b1, b2, eps, vec);
+  auto k = weight_decay != 0.f ? adam_step_kernel<true> : adam_step_kernel<false>;
+  k<<<stream_grid(vec ? (n + 3) / 4 : n), 256, 0, st>>>(p, g, m, v, normsq, step_t, norm_out, n, max_norm, lr, b1, b2, eps,
+                                                        weight_decay, vec);
   RL_CHECK_LAUNCH();
   return B200RL_OK;
+}
+
+extern "C" int b200rl_adam_step(float* p, const float* g, float* m, float* v, const double* normsq, const int* step_t,
+                                float* norm_out, long long n, float max_norm, float lr, float b1, float b2, float eps,
+                                cudaStream_t st) {
+  return b200rl_adam_step_wd(p, g, m, v, normsq, step_t, norm_out, n, max_norm, lr, b1, b2, eps, 0.f, st);
 }
 
 extern "C" int b200rl_rmsprop_step(float* p, const float* g, float* square_avg, float* momentum_buf, float* grad_avg,

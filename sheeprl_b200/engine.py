@@ -468,10 +468,11 @@ class DV3Engine:
         return self.cuda_graph and self.device.type == "cuda" and type(self.ops).__name__ == "CudaOps"
 
     def graph_key(self) -> tuple:
-        """what a captured step bakes in besides the batch shapes: the learning rates (kernel arguments by value)"""
+        """what a captured step bakes in besides the batch shapes: the learning rates and weight decays (kernel arguments
+        by value)"""
         prec = self.ops.matmul_precision() if hasattr(self.ops, "matmul_precision") else "highest"
-        return tuple(float(g.optimizer.lr) if getattr(g, "optimizer", None) is not None else -1.0
-                     for g in self.optimizer_groups()) + (prec,)
+        return tuple((float(g.optimizer.lr), g.adam_kwargs().get("weight_decay", 0.0))
+                     if getattr(g, "optimizer", None) is not None else -1.0 for g in self.optimizer_groups()) + (prec,)
 
     def step_graph(self):
         if self._graph is None:
@@ -1034,7 +1035,8 @@ class DV3Engine:
         opt = getattr(g, "optimizer", None)                  # the handle build by main / make_optimizers (schedulers edit it)
         lr = opt.lr if opt is not None else float(ocfg.lr)
         ops.adam_step(g.flat, g.grad, g.exp_avg, g.exp_avg_sq, self.normsq[name], max_norm, lr,
-                      float(b1), float(b2), float(ocfg.eps), g.step_t, self.norms[slot: slot + 1])
+                      float(b1), float(b2), float(ocfg.eps), g.step_t, self.norms[slot: slot + 1],
+                      **g.adam_kwargs(ocfg.get("weight_decay", 0.0)))
 
     # ------------------------------------------------------------------ behaviour learning
     def _actor_heads(self, hidden: torch.Tensor, raw_out: torch.Tensor, actor: Optional[FlatGroup] = None):

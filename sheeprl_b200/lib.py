@@ -416,11 +416,12 @@ class CudaOps:
         assert out.dtype == torch.float64 and x.is_contiguous()
         self._ck(self.lib.b200rl_sumsq(_p(x), x.numel(), _p(out), self._st()))
 
-    def adam_step(self, p, g, m, v, normsq, max_norm, lr, b1, b2, eps, step_t, norm_out):
+    def adam_step(self, p, g, m, v, normsq, max_norm, lr, b1, b2, eps, step_t, norm_out, weight_decay=0.0):
+        """clip + torch.optim.Adam; weight_decay is torch's L2 term, added to the clipped gradient"""
         _f32(p, g, m, v, norm_out)
         assert step_t.dtype == torch.int32 and normsq.dtype == torch.float64
-        self._ck(self.lib.b200rl_adam_step(_p(p), _p(g), _p(m), _p(v), _p(normsq), _p(step_t), _p(norm_out), p.numel(),
-                                           max_norm, lr, b1, b2, eps, self._st()))
+        self._ck(self.lib.b200rl_adam_step_wd(_p(p), _p(g), _p(m), _p(v), _p(normsq), _p(step_t), _p(norm_out),
+                                              p.numel(), max_norm, lr, b1, b2, eps, weight_decay, self._st()))
 
     def rmsprop_step(self, p, g, square_avg, momentum_buf, grad_avg, normsq, max_norm, lr, alpha, eps, weight_decay,
                      momentum, norm_out):

@@ -71,3 +71,11 @@ class FlatGroup:
         if self.grad_avg is None:
             self.grad_avg = torch.zeros_like(self.flat)
         return self.grad_avg
+
+    def adam_kwargs(self, weight_decay: float = 0.0) -> dict:
+        """`ops.adam_step`'s optional arguments: the L2 weight decay of the optimizer handle attached to this group
+        (`B200Adam`, built from the same optimizer config), or `weight_decay` when no handle is attached.  Without decay
+        the call keeps the plain Adam form."""
+        opt = getattr(self, "optimizer", None)
+        wd = float((opt.param_groups[0].get("weight_decay") if opt is not None else weight_decay) or 0.0)
+        return {"weight_decay": wd} if wd else {}
