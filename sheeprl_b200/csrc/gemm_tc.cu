@@ -212,7 +212,10 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                const float* __restrict__ bias, int M, int N, int K, int ldc, int accumulate, const TileGeo geo) {
   constexpr int STAGES = Smem<BN>::STAGES;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  Smem<BN>& s = *reinterpret_cast<Smem<BN>*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  // Align by offsetting the shared array itself (not by integer arithmetic on its generic address), so that the compiler
+  // still knows every access through `s` is to shared memory: the consumers' A-fragment loads and the splitters' B
+  // loads / stores become 32-bit-addressed LDS / STS instead of generic 64-bit LD / ST.
+  Smem<BN>& s = *reinterpret_cast<Smem<BN>*>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int mtiles = geo.mtiles * geo.ntiles, tstride = gridDim.y;   // flattened tile count
   auto tile_mn = [&](int id, int& tm, int& tn) {
@@ -307,6 +310,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         const char* raw = reinterpret_cast<const char*>(s.b[st]);
         char* bh = reinterpret_cast<char*>(s.b_hi[st]);
         char* bl = reinterpret_cast<char*>(s.b_lo[st]);
+        // ~11 work items per thread: unrolled so that several items' loads are in flight before their stores
+#pragma unroll 4
         for (int w = t; w < BN * BK / 4; w += NSPLIT_THREADS) {
           // work item = one 16-byte chunk (row n, k = 4kc .. 4kc+3) of the K-major target.  MN-major source: a warp
           // covers 32 consecutive n of one kc, so every gather load reads one 128-byte line (conflict-free)
