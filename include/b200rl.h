@@ -305,6 +305,34 @@ int b200rl_sac_actor_loss(const float* q, long long stride_net, int nets, const 
 int b200rl_fill_normal(float* out, long long n, unsigned long long seed, unsigned int stream_id, const int* counter_dev,
                        cudaStream_t stream);
 
+/* ---- DroQ critics (csrc/droq.cu) ----------------------------------------------------------------------------
+ * DroQ's policy loss: b200rl_sac_actor_loss with the mean over the critics in place of the min (droq/droq.py:147-150):
+ * actor_loss = mean(alpha*logp - mean_n q[n]), dq[n,b] = -1/(nets*B); alpha loss and its gradient as SAC's. */
+int b200rl_droq_actor_loss(const float* q, long long stride_net, int nets, const float* logp, const float* log_alpha,
+                           float target_entropy, float* dq, float* actor_loss, float* alpha_loss, float* dlog_alpha,
+                           int B, cudaStream_t stream);
+/* nn.Dropout's keep masks (Bernoulli(1-p), droq/agent.py:40-42) for n_words 32-bit words, bit-packed: a [n, B, H]
+ * activation takes [n, B, ceil(H/32)] words, bit j of word k keeping column 32k + j.  Philox4x32-10 keyed by (seed,
+ * stream_id, *counter_dev) as b200rl_fill_normal, so one launch fills the masks of every critic forward of a train()
+ * call without a host synchronisation. */
+int b200rl_dropout_mask(unsigned int* mask, long long n_words, float p, unsigned long long seed, unsigned int stream_id,
+                        const int* counter_dev, cudaStream_t stream);
+/* The miniblock after each hidden Linear of the DroQ critic (utils/model.py:34-88: Dropout(p) -> LayerNorm(H, eps) ->
+ * ReLU) for all `nets` critics in one launch: y = relu(LN(z * mask / (1-p)) * gamma + beta).  z, y [nets, B, H]
+ * contiguous; mask [nets, B, ceil(H/32)] words (NULL iff p == 0; bits past column H are never read); gamma / beta of
+ * critic i at i * stride_param; stats [nets, B, 2] = (mean, 1/std) per row, kept for the backward.  1 <= H <= 1024:
+ * `_supported` answers for H. */
+int b200rl_dropout_ln_relu_supported(int H);
+int b200rl_dropout_ln_relu_fwd(const float* z, const unsigned int* mask, float p, const float* gamma, const float* beta,
+                               long long stride_param, float eps, float* y, float* stats, int nets, int B, int H,
+                               cudaStream_t stream);
+/* its autograd backward: dReLU, LayerNorm backward, then the mask scale, giving dz [nets, B, H] from dy.  dgamma / dbeta
+ * (both or neither, same stride as gamma) are reduced over the rows in a fixed order, bit-identical run to run; NULL
+ * gives the input-gradient-only pass of the policy loss. */
+int b200rl_dropout_ln_relu_bwd(const float* dy, const float* y, const float* z, const unsigned int* mask, float p,
+                               const float* stats, const float* gamma, long long stride_param, float* dz, float* dgamma,
+                               float* dbeta, int nets, int B, int H, cudaStream_t stream);
+
 /* ---- PPO --------------------------------------------------------------------------------------------------
  * Channel-last patch gather / scatter for NatureCNN's unpadded convolutions (models/models.py:288-328):
  * col[(b,oy,ox),(ky,kx,c)] = x[b,oy*s+ky,ox*s+kx,c]; col2im is its transpose (sum over overlapping patches), optionally

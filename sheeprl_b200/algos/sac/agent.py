@@ -116,6 +116,9 @@ class SACPlayer:
 
     __call__ = forward = get_actions
 
+    def eval(self):  # the reference's test loop (sac/utils.py:test) switches the player to inference mode
+        return self
+
 
 def build_agent(fabric, cfg: Dict[str, Any], obs_space, action_space, agent_state: Optional[Dict[str, torch.Tensor]] = None,
                 ops=None) -> Tuple[SACAgent, SACPlayer]:

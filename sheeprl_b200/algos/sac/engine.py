@@ -49,7 +49,7 @@ class SACEngine:
         self.target_entropy = -float(act_dim)                               # sac/agent.py:341
         self.device, self.ops = torch.device(device), ops
         self.opt = {"actor": opt_actor, "qf": opt_qf, "alpha": opt_alpha}
-        sa, sq = sac_param_shapes(obs_dim, act_dim, hidden_actor, hidden_critic, n_critics)
+        sa, sq = self._param_shapes()
         self.actor = FlatGroup(sa, device)
         self.qf = FlatGroup(sq, device)
         self.qf_target = FlatGroup(sq, device, with_optimizer=False)
@@ -67,6 +67,9 @@ class SACEngine:
         self.noise_counter = torch.zeros(1, dtype=torch.int32, device=self.device)
         self.metrics = torch.zeros(3, dtype=torch.float32, device=self.device)      # value, policy, alpha loss
         self._alloc()
+
+    def _param_shapes(self):
+        return sac_param_shapes(self.O, self.A, self.Ha, self.Hc, self.n)
 
     # ------------------------------------------------------------------ buffers
     def _alloc(self):
@@ -149,7 +152,6 @@ class SACEngine:
         o.copy(obs, self.x_pi[:, :O])
         o.copy(data["actions"], self.x_cur[:, O:])
         la = self.alpha.views["log_alpha"]
-        t = lambda W: W.transpose(1, 2)  # noqa: E731
         # ---- soft-critic update (sac.py:45-53)
         self._actor_fwd(nobs, eps_next, self.x_next[:, O:], save_tanh=False)
         self._critic_fwd(self._tv, self.x_next)
@@ -157,21 +159,21 @@ class SACEngine:
                      self.gamma, self.y)
         self._critic_fwd(self._qv, self.x_cur)
         o.sac_critic_loss(self.q[:, :, 0], self.y, self.dq[:, :, 0], self.metrics[0:1])
-        w, g = self._qv, self._qg
-        self._critic_bwd_weights(w, g, self.x_cur)
+        self._critic_bwd_weights(self._qv, self._qg, self.x_cur)
         self._adam(self.qf, self.opt["qf"], "qf")
         # ---- target EMA (sac.py:55-57)
         if do_ema:
             o.ema(self.qf_target.flat, self.qf.flat, self.tau)
-        # ---- actor update (sac.py:59-66)
+        # ---- actor update (sac.py:59-66) and temperature (sac.py:68-73)
+        self._actor_update(obs, eps_cur)
+
+    def _actor_update(self, obs: torch.Tensor, eps_cur: torch.Tensor):
+        """one actor and one temperature step on `obs` (whose copy already sits in x_pi's observation columns)"""
+        o, O = self.ops, self.O
+        la = self.alpha.views["log_alpha"]
+        t = lambda W: W.transpose(1, 2)  # noqa: E731
         self._actor_fwd(obs, eps_cur, self.x_pi[:, O:], save_tanh=True)
-        self._critic_fwd(self._qv, self.x_pi)
-        o.sac_actor_loss(self.q[:, :, 0], self.logp, la, self.target_entropy, self.dq[:, :, 0], self.metrics[1:2],
-                         self.metrics[2:3], self.alpha.grad[0:1])
-        # input gradient of the critics w.r.t. the action columns only
-        o.bgemm(self.dq, w["W2"], self.dc2, aux=self.c2, epi="drelu")
-        o.bgemm(self.dc2, w["W1"], self.dc1, aux=self.c1, epi="drelu")
-        o.bgemm(self.dc1, w["W0"][:, :, O:], self.dact)
+        self._policy_loss_grad()
         o.sac_sample_bwd(self.head[0], eps_cur, self.tanh_y, self.scale, self.dact, la, self.dhead[0])
         aw, ag = self._actor_views(self.actor.views), self._actor_views(self.actor.gviews)
         o.bgemm(t(self.dhead), self.a2, ag["W2"], rsum=ag["b2"])
@@ -180,8 +182,20 @@ class SACEngine:
         o.bgemm(self.da2, aw["W1"], self.da1, aux=self.a1, epi="drelu")
         o.bgemm(t(self.da1), obs.unsqueeze(0), ag["W0"], rsum=ag["b0"])
         self._adam(self.actor, self.opt["actor"], "actor")
-        # ---- temperature (sac.py:68-73): gradient written by sac_actor_loss
+        # temperature: gradient written by the policy loss kernel
         self._adam(self.alpha, self.opt["alpha"], "alpha")
+
+    def _policy_loss_grad(self):
+        """policy + temperature losses on the critics' q of x_pi (min over the critics), dq, the log_alpha gradient and
+        the input gradient of the critics w.r.t. the action columns only (dact)"""
+        o, O, w = self.ops, self.O, self._qv
+        la = self.alpha.views["log_alpha"]
+        self._critic_fwd(w, self.x_pi)
+        o.sac_actor_loss(self.q[:, :, 0], self.logp, la, self.target_entropy, self.dq[:, :, 0], self.metrics[1:2],
+                         self.metrics[2:3], self.alpha.grad[0:1])
+        o.bgemm(self.dq, w["W2"], self.dc2, aux=self.c2, epi="drelu")
+        o.bgemm(self.dc2, w["W1"], self.dc1, aux=self.c1, epi="drelu")
+        o.bgemm(self.dc1, w["W0"][:, :, O:], self.dact)
 
     def _critic_bwd_weights(self, w, g, x):
         o = self.ops

@@ -85,4 +85,12 @@ __device__ __forceinline__ float signf_(float x) { return (x > 0.f) ? 1.f : ((x 
 __device__ __forceinline__ float symlogf_(float x) { return signf_(x) * logf(1.f + fabsf(x)); }
 __device__ __forceinline__ float symexpf_(float x) { return signf_(x) * (expf(fabsf(x)) - 1.f); }
 
+// one round of Philox4x32-10 (the noise fills key c = {index lo, index hi, stream id, device counter} by the seed)
+__device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
+  const uint32_t hi0 = __umulhi(0xD2511F53u, c[0]), lo0 = 0xD2511F53u * c[0];
+  const uint32_t hi1 = __umulhi(0xCD9E8D57u, c[2]), lo1 = 0xCD9E8D57u * c[2];
+  const uint32_t n0 = hi1 ^ c[1] ^ k0, n1 = lo1, n2 = hi0 ^ c[3] ^ k1, n3 = lo0;
+  c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
+}
+
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }

@@ -195,14 +195,6 @@ __global__ void ema_kernel(float* __restrict__ tgt, const float* __restrict__ sr
   for (long long i = done + tid; i < n; i += stride) tgt[i] = tgt[i] * (1.f - tau) + tau * src[i];
 }
 
-// Philox4x32-10
-__device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
-  const uint32_t hi0 = __umulhi(0xD2511F53u, c[0]), lo0 = 0xD2511F53u * c[0];
-  const uint32_t hi1 = __umulhi(0xCD9E8D57u, c[2]), lo1 = 0xCD9E8D57u * c[2];
-  const uint32_t n0 = hi1 ^ c[1] ^ k0, n1 = lo1, n2 = hi0 ^ c[3] ^ k1, n3 = lo0;
-  c[0] = n0; c[1] = n1; c[2] = n2; c[3] = n3;
-}
-
 __global__ void fill_exponential_kernel(float* __restrict__ out, long long n, uint32_t seed_lo, uint32_t seed_hi,
                                         uint32_t stream, const int* __restrict__ counter) {
   const uint32_t ctr = counter ? (uint32_t)(*counter) : 0u;  // device-side call counter (CUDA-graph safe)

@@ -2,7 +2,8 @@
 //
 // Replaces (reference): SACActor._get_actions_and_log_probs sheeprl/algos/sac/agent.py:110-142 (+ its autograd
 // backward), SACAgent.get_next_target_q_values agent.py:254-262, critic_loss / policy_loss / entropy_loss
-// sheeprl/algos/sac/loss.py:9-29 and the `.mean()` / `torch.min` glue of train() sheeprl/algos/sac/sac.py:45-73.
+// sheeprl/algos/sac/loss.py:9-29 and the `.mean()` / `torch.min` glue of train() sheeprl/algos/sac/sac.py:45-73; DroQ's
+// policy loss over the mean of its critics (sheeprl/algos/droq/droq.py:147-150).
 // The temperature is read from the device-resident log_alpha (the reference does `.exp().item()`: a host sync per
 // use), so a whole update can sit in one CUDA graph.  B <= a few thousand rows: single-CTA reductions.
 #include "common.cuh"
@@ -93,8 +94,10 @@ sac_critic_loss_kernel(const float* __restrict__ q, long long stride_net, int ne
   if (threadIdx.x == 0) loss_out[0] = acc * invB;
 }
 
-// actor_loss = mean(alpha*logp - min_n q[n]) ; dq[n,b] = -1/B at the arg-min critic (first on ties, as torch.min)
+// actor_loss = mean(alpha*logp - Q) with Q = min_n q[n] (SAC) or mean_n q[n] (DroQ, droq.py:147-150).
+// min: dq[n,b] = -1/B at the arg-min critic (first on ties, as torch.min); mean: dq[n,b] = -1/(nets*B) for every critic.
 // alpha_loss = mean(-log_alpha * (logp + target_entropy)) ; d/dlog_alpha = -mean(logp + target_entropy)
+template <bool kMeanOverCritics>
 __global__ void __launch_bounds__(256)
 sac_actor_loss_kernel(const float* __restrict__ q, long long stride_net, int nets, const float* __restrict__ logp,
                       const float* __restrict__ log_alpha, float target_entropy, float* __restrict__ dq,
@@ -105,12 +108,19 @@ sac_actor_loss_kernel(const float* __restrict__ q, long long stride_net, int net
   float s_actor = 0.f, s_ent = 0.f;
   for (int b = threadIdx.x; b < B; b += blockDim.x) {
     float m = q[b];
-    int arg = 0;
-    for (int n = 1; n < nets; ++n) {
-      const float v = q[n * stride_net + b];
-      if (v < m) { m = v; arg = n; }
+    if (kMeanOverCritics) {
+      const float inv_nets = 1.f / (float)nets;
+      for (int n = 1; n < nets; ++n) m += q[n * stride_net + b];
+      m *= inv_nets;
+      for (int n = 0; n < nets; ++n) dq[n * stride_net + b] = -invB * inv_nets;
+    } else {
+      int arg = 0;
+      for (int n = 1; n < nets; ++n) {
+        const float v = q[n * stride_net + b];
+        if (v < m) { m = v; arg = n; }
+      }
+      for (int n = 0; n < nets; ++n) dq[n * stride_net + b] = (n == arg) ? -invB : 0.f;
     }
-    for (int n = 0; n < nets; ++n) dq[n * stride_net + b] = (n == arg) ? -invB : 0.f;
     s_actor += alpha * logp[b] - m;
     s_ent += logp[b] + target_entropy;
   }
@@ -167,13 +177,28 @@ extern "C" int b200rl_sac_critic_loss(const float* q, long long stride_net, int 
   return B200RL_OK;
 }
 
+template <bool kMeanOverCritics>
+static int actor_loss_launch(const float* q, long long stride_net, int nets, const float* logp, const float* log_alpha,
+                             float target_entropy, float* dq, float* actor_loss, float* alpha_loss, float* dlog_alpha,
+                             int B, cudaStream_t st) {
+  RL_CHECK_ARG(q && logp && log_alpha && dq && actor_loss && alpha_loss && dlog_alpha, "null pointer");
+  RL_CHECK_ARG(B > 0 && nets > 0, "bad dims");
+  sac_actor_loss_kernel<kMeanOverCritics><<<1, 256, 0, st>>>(q, stride_net, nets, logp, log_alpha, target_entropy, dq,
+                                                             actor_loss, alpha_loss, dlog_alpha, B);
+  RL_CHECK_LAUNCH();
+  return B200RL_OK;
+}
+
 extern "C" int b200rl_sac_actor_loss(const float* q, long long stride_net, int nets, const float* logp,
                                      const float* log_alpha, float target_entropy, float* dq, float* actor_loss,
                                      float* alpha_loss, float* dlog_alpha, int B, cudaStream_t st) {
-  RL_CHECK_ARG(q && logp && log_alpha && dq && actor_loss && alpha_loss && dlog_alpha, "null pointer");
-  RL_CHECK_ARG(B > 0 && nets > 0, "bad dims");
-  sac_actor_loss_kernel<<<1, 256, 0, st>>>(q, stride_net, nets, logp, log_alpha, target_entropy, dq, actor_loss,
-                                           alpha_loss, dlog_alpha, B);
-  RL_CHECK_LAUNCH();
-  return B200RL_OK;
+  return actor_loss_launch<false>(q, stride_net, nets, logp, log_alpha, target_entropy, dq, actor_loss, alpha_loss,
+                                  dlog_alpha, B, st);
+}
+
+extern "C" int b200rl_droq_actor_loss(const float* q, long long stride_net, int nets, const float* logp,
+                                      const float* log_alpha, float target_entropy, float* dq, float* actor_loss,
+                                      float* alpha_loss, float* dlog_alpha, int B, cudaStream_t st) {
+  return actor_loss_launch<true>(q, stride_net, nets, logp, log_alpha, target_entropy, dq, actor_loss, alpha_loss,
+                                 dlog_alpha, B, st);
 }

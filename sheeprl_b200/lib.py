@@ -621,6 +621,50 @@ class CudaOps:
         _f32(out)
         self._ck(self.lib.b200rl_fill_normal(_p(out), out.numel(), seed, stream_id, _p(counter), self._st()))
 
+    # ------------------------------------------------------------------ DroQ critics (csrc/droq.cu)
+    def droq_actor_loss(self, q, logp, log_alpha, target_entropy: float, dq, actor_loss, alpha_loss, dlog_alpha):
+        """sac_actor_loss with the mean over the critics in place of the min"""
+        _f32(q, logp, log_alpha, dq, actor_loss, alpha_loss, dlog_alpha)
+        nets, B = q.shape
+        assert q.is_contiguous() and dq.is_contiguous()
+        self._ck(self.lib.b200rl_droq_actor_loss(_p(q), B, nets, _p(logp), _p(log_alpha), target_entropy, _p(dq),
+                                                 _p(actor_loss), _p(alpha_loss), _p(dlog_alpha), B, self._st()))
+
+    def dropout_mask(self, mask, p: float, seed: int, stream_id: int, counter=None):
+        """mask: int32 words, bit-packed keep masks (`[..., ceil(H/32)]` per [..., H] activation)"""
+        assert mask.dtype == torch.int32 and mask.is_cuda and mask.is_contiguous()
+        self._ck(self.lib.b200rl_dropout_mask(_p(mask), mask.numel(), p, seed, stream_id, _p(counter), self._st()))
+
+    def dropout_ln_relu_supported(self, H: int) -> bool:
+        return bool(self.lib.b200rl_dropout_ln_relu_supported(H))
+
+    @staticmethod
+    def _dln_args(z, mask, gamma, stats):
+        nets, B, H = z.shape
+        assert z.is_contiguous() and stats.is_contiguous() and stats.shape == (nets, B, 2)
+        assert gamma.shape == (nets, H) and (H == 1 or gamma.stride(1) == 1)
+        if mask is not None:
+            assert mask.dtype == torch.int32 and mask.is_contiguous() and mask.shape == (nets, B, (H + 31) // 32)
+        return nets, B, H, (gamma.stride(0) if nets > 1 else H)
+
+    def dropout_ln_relu_fwd(self, z, mask, p: float, gamma, beta, eps: float, y, stats):
+        """y = relu(LayerNorm(z * mask / (1-p))) for all critics; z, y [n, B, H]; gamma / beta [n, H] strided views"""
+        _f32(z, gamma, beta, y, stats)
+        nets, B, H, sp = self._dln_args(z, mask, gamma, stats)
+        assert y.shape == z.shape and y.is_contiguous() and beta.stride() == gamma.stride()
+        self._ck(self.lib.b200rl_dropout_ln_relu_fwd(_p(z), _p(mask), p, _p(gamma), _p(beta), sp, eps, _p(y), _p(stats),
+                                                     nets, B, H, self._st()))
+
+    def dropout_ln_relu_bwd(self, dy, y, z, mask, p: float, stats, gamma, dz, dgamma=None, dbeta=None):
+        _f32(dy, y, z, stats, gamma, dz, dgamma, dbeta)
+        nets, B, H, sp = self._dln_args(z, mask, gamma, stats)
+        for t in (dy, y, dz):
+            assert t.shape == z.shape and t.is_contiguous()
+        for t in (dgamma, dbeta):
+            assert t is None or t.stride() == gamma.stride()
+        self._ck(self.lib.b200rl_dropout_ln_relu_bwd(_p(dy), _p(y), _p(z), _p(mask), p, _p(stats), _p(gamma), sp,
+                                                     _p(dz), _p(dgamma), _p(dbeta), nets, B, H, self._st()))
+
     # ------------------------------------------------------------------ PPO (csrc/ppo.cu)
     def im2col(self, x, col, k: int, stride: int):
         """x [B,H,W,C] channel-last -> col [B*Ho*Wo, k*k*C]"""
