@@ -50,6 +50,20 @@ int b200rl_gemm_tc_supported(const float* A, const float* B, int M, int N, int K
                              int transB);
 int b200rl_gemm_tc(const float* A, const float* B, float* C, const float* bias, int M, int N, int K, int lda, int ldb,
                    int ldc, int transA, int transB, int accumulate, cudaStream_t stream);
+/* Weight operands split once, before the products that read them: X = hi + lo exactly, hi = X with the 13 low mantissa
+ * bits cleared (what the TF32 datapath keeps), lo = X - hi.  b200rl_tf32_split: elementwise over n floats.
+ * b200rl_tf32_split_t: W [rows][cols] (ldw) -> hi^T, lo^T [cols][ldt], columns [rows, ldt) zeroed (ldt a multiple of 4 so
+ * that TMA can address the rows). */
+int b200rl_tf32_split(const float* X, float* Xhi, float* Xlo, long long n, cudaStream_t stream);
+int b200rl_tf32_split_t(const float* W, float* Thi, float* Tlo, int rows, int cols, long long ldw, long long ldt,
+                        cudaStream_t stream);
+/* C = A B^T (+bias) (+C) with B [N][K] given as its TF32 planes (row stride ldb each): the kernel loads them straight into
+ * its operand stages instead of splitting B per tile.  Bit-identical to b200rl_gemm_tc(transA = 0, transB = 1) on
+ * B = Bhi + Blo. */
+int b200rl_gemm_tc_presplit_supported(const float* A, const float* Bhi, const float* Blo, int M, int N, int K, int lda,
+                                      int ldb);
+int b200rl_gemm_tc_presplit(const float* A, const float* Bhi, const float* Blo, float* C, const float* bias, int M, int N,
+                            int K, int lda, int ldb, int ldc, int accumulate, cudaStream_t stream);
 /* Dense block Linear(bias=False) -> LayerNorm(eps) -> activation in two launches (sheeprl/utils/model.py:34-88 miniblock,
  * as built by MLP at sheeprl/models/models.py:23-119): the wgmma product leaves split-K partial tiles, one kernel sums
  * them in split order, normalises the row in registers and applies the activation.  `pre` (optional) keeps W.x for the
@@ -62,6 +76,13 @@ int b200rl_gemm_ln(const float* A, const float* W, int M, int N, int K, int lda,
                    const float* beta, float eps, int act, float* pre, long long ldpre, float* out, long long ldout,
                    int mode, const float* h_prev, long long ldh, float* h_out, long long ldho, float* h_out2,
                    long long ldho2, cudaStream_t stream);
+/* The same with W given as its TF32 planes (b200rl_tf32_split); bit-identical to b200rl_gemm_ln on W = Whi + Wlo. */
+int b200rl_gemm_ln_presplit_supported(const float* A, const float* Whi, const float* Wlo, int M, int N, int K, int lda,
+                                      int ldw, int mode);
+int b200rl_gemm_ln_presplit(const float* A, const float* Whi, const float* Wlo, int M, int N, int K, int lda, int ldw,
+                            const float* gamma, const float* beta, float eps, int act, float* pre, long long ldpre,
+                            float* out, long long ldout, int mode, const float* h_prev, long long ldh, float* h_out,
+                            long long ldho, float* h_out2, long long ldho2, cudaStream_t stream);
 /* nn.LayerNorm(eps) (+ nn.SiLU): miniblock sheeprl/utils/model.py:34-88; LayerNormChannelLast
  * sheeprl/models/models.py:507-518 (channel-last is native here).  act: 0 none, 1 SiLU, 2 tanh, 3 ReLU (the last two:
  * PPO MLPs with layer_norm=True, sheeprl/algos/ppo/agent.py:58-66,152-176). */
@@ -115,6 +136,13 @@ int b200rl_conv_down_tc(const float* big, const float* Wpacked, float* small_, i
                         cudaStream_t stream);
 int b200rl_conv_up_tc(const float* small_, const float* Wpacked, float* big, const float* bias, int NB, int h, int w,
                       int Cs, int Cb, cudaStream_t stream);
+/* The packed weight as its TF32 planes (two workspaces of b200rl_conv_pack_floats() floats each), and the conv forwards
+ * that read them; bit-identical to b200rl_conv_pack + b200rl_conv_down_tc / _up_tc. */
+int b200rl_conv_pack_split(const float* W, float* Whi, float* Wlo, int mode_up, int Cs, int Cb, cudaStream_t stream);
+int b200rl_conv_down_tc_presplit(const float* big, const float* Whi, const float* Wlo, float* small_, int NB, int h, int w,
+                                 int Cs, int Cb, cudaStream_t stream);
+int b200rl_conv_up_tc_presplit(const float* small_, const float* Whi, const float* Wlo, float* big, const float* bias,
+                               int NB, int h, int w, int Cs, int Cb, cudaStream_t stream);
 
 /* ---- RSSM ------------------------------------------------------------------------------------------
  * LayerNormGRUCell gates models.py:399-403; is_first masking agent.py:425-430; unimix agent.py:437-449;

@@ -43,8 +43,13 @@ constexpr int NCONS_WARPS = 8;                      // warpgroups 1 and 2
 // register budget per thread after setmaxnreg: the producer warpgroup gives its registers to the consumers, which hold
 // the chunk accumulator, the running fp32 sum and the A fragments of a stage (128 x BN tile: up to 64 + 64 + 32)
 constexpr int PRODUCER_REGS = 56, CONSUMER_REGS = 224;
-// operand stages that fit the 227 KB of shared memory: raw A, raw B, B hi, B lo per stage
-template <int BN> constexpr int stages_for() { return BN == 128 ? 3 : 5; }
+// Operand stages that fit the 227 KB of shared memory (less the 1024-byte alignment slack and the barriers).  A raw-B
+// stage holds raw A, raw B, B hi and B lo; a pre-split stage holds raw A and the B planes TMA loads straight into the
+// wgmma operand buffers (hi and lo; hi only in a single-pass product).
+template <int PASSES, bool PRESPLIT> __host__ __device__ constexpr int b_buffers() { return PRESPLIT ? (PASSES == 3 ? 2 : 1) : 3; }
+template <int BN, int PASSES, bool PRESPLIT> constexpr int stages_for() {
+  return (227 * 1024 - 1024 - 256) / ((BM + b_buffers<PASSES, PRESPLIT>() * BN) * BK * (int)sizeof(float));
+}
 
 // ---------------------------------------------------------------- PTX wrappers
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -160,15 +165,26 @@ __device__ __forceinline__ uint32_t mnmajor_off(int r, int k) {
   return (uint32_t)((r >> 5) * 4096 + k * 128 + (((((r & 31) >> 2) ^ k) & 7) << 4) + (r & 3) * 4);
 }
 
-template <int BN>
-struct Smem {
-  static constexpr int STAGES = stages_for<BN>();
+template <int BN, int PASSES, bool PRESPLIT>
+struct Smem;
+template <int BN, int PASSES>
+struct Smem<BN, PASSES, false> {
+  static constexpr int STAGES = stages_for<BN, PASSES, false>();
   // every operand buffer is a whole number of 1024-byte swizzle groups
   float a[STAGES][BM * BK];      // raw A tiles (the consumers split them in registers)
   float b[STAGES][BN * BK];      // raw B tiles
   float b_hi[STAGES][BN * BK];   // K-major hi / lo halves of B, the wgmma operands
   float b_lo[STAGES][BN * BK];
   uint64_t full[STAGES], split[STAGES], empty[STAGES];
+};
+// B given as its K-major TF32 hi / lo planes: TMA fills the wgmma operand buffers directly (no b_lo at PASSES == 1)
+template <int BN, int PASSES>
+struct Smem<BN, PASSES, true> {
+  static constexpr int STAGES = stages_for<BN, PASSES, true>();
+  float a[STAGES][BM * BK];
+  float b_hi[STAGES][BN * BK];
+  float b_lo[PASSES == 3 ? STAGES : 1][PASSES == 3 ? BN * BK : 256];
+  uint64_t full[STAGES], empty[STAGES];
 };
 
 // Two-level accumulation.  The tensor core adds each k-step into its fp32 accumulator with truncation
@@ -206,16 +222,21 @@ struct TileGeo {
                            // from the channel-last big image by 4-D TMA boxes of 32 pixels (Cout = big channels)
 };
 
-template <int BN, int PASSES>
+// PRESPLIT: B arrives as K-major TF32 hi / lo planes (mapB / mapBlo, [N][K]) that TMA loads into the wgmma operand
+// buffers; warps 1-3 idle and the consumers wait on `full` alone.  Otherwise mapB is raw B (K- or MN-major, per geo.b_mn)
+// and the splitters write its halves (mapBlo unused).
+template <int BN, int PASSES, bool PRESPLIT>
 __global__ void __launch_bounds__(NTHREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, float* __restrict__ C,
-               const float* __restrict__ bias, int M, int N, int K, int ldc, int accumulate, const TileGeo geo) {
-  constexpr int STAGES = Smem<BN>::STAGES;
+gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB,
+               const __grid_constant__ CUtensorMap mapBlo, float* __restrict__ C, const float* __restrict__ bias, int M,
+               int N, int K, int ldc, int accumulate, const TileGeo geo) {
+  using S = Smem<BN, PASSES, PRESPLIT>;
+  constexpr int STAGES = S::STAGES;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   // Align by offsetting the shared array itself (not by integer arithmetic on its generic address), so that the compiler
   // still knows every access through `s` is to shared memory: the consumers' A-fragment loads and the splitters' B
   // loads / stores become 32-bit-addressed LDS / STS instead of generic 64-bit LD / ST.
-  Smem<BN>& s = *reinterpret_cast<Smem<BN>*>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
+  S& s = *reinterpret_cast<S*>(smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int mtiles = geo.mtiles * geo.ntiles, tstride = gridDim.y;   // flattened tile count
   auto tile_mn = [&](int id, int& tm, int& tn) {
@@ -244,7 +265,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&s.full[i], 1);
-      mbar_init(&s.split[i], NSPLIT_THREADS / 32);
+      if constexpr (!PRESPLIT) mbar_init(&s.split[i], NSPLIT_THREADS / 32);
       mbar_init(&s.empty[i], NCONS_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -256,6 +277,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
     if (warp == 0) {
       // ===== TMA producer.  The whole warp walks the loop with warp-uniform control flow; the elected lane issues.
       const bool leader = elect_one();
+      constexpr uint32_t STAGE_TX = (uint32_t)((BM + (PRESPLIT ? b_buffers<PASSES, true>() : 1) * BN) * BK * sizeof(float));
+      // the stage's K-major B tile(s) at (k, n): raw B, or the hi (and lo) planes
+      auto load_b_kmajor = [&](int st, int k, int n) {
+        if constexpr (PRESPLIT) {
+          tma_load_2d(s.b_hi[st], &mapB, &s.full[st], k, n);
+          if (PASSES == 3) tma_load_2d(s.b_lo[st], &mapBlo, &s.full[st], k, n);
+        } else {
+          tma_load_2d(s.b[st], &mapB, &s.full[st], k, n);
+        }
+      };
       int it = 0;                                  // k-blocks issued so far, across tiles: stage / phase bookkeeping
       for (int tile = blockIdx.y; tile < mtiles; tile += tstride) {
         int tm, tn;
@@ -267,7 +298,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
           const int st = it % STAGES;
           if (it >= STAGES) mbar_wait(&s.empty[st], ((it / STAGES) - 1) & 1);
           if (leader) {
-            mbar_expect_tx(&s.full[st], (uint32_t)((BM + BN) * BK * sizeof(float)));
+            mbar_expect_tx(&s.full[st], STAGE_TX);
             if (geo.mode == MODE_GEMM) {
               const int k0 = (kb_base + kb) * BK;
               if (geo.wg) {
@@ -281,8 +312,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
               } else if (!geo.a_mn) tma_load_2d(s.a[st], &mapA, &s.full[st], k0, m0);
               else
                 for (int j = 0; j < BM / 32; ++j) tma_load_2d(s.a[st] + j * 1024, &mapA, &s.full[st], m0 + 32 * j, k0);
-              if (!geo.b_mn) tma_load_2d(s.b[st], &mapB, &s.full[st], k0, n0);
-              else
+              if (PRESPLIT || !geo.b_mn) load_b_kmajor(st, k0, n0);
+              else if constexpr (!PRESPLIT)
                 for (int j = 0; j < BN / 32; ++j) tma_load_2d(s.b[st] + j * 1024, &mapB, &s.full[st], n0 + 32 * j, k0);
             } else {
               const int tap = kb / geo.chunks, ch = (kb - tap * geo.chunks) * BK;
@@ -291,13 +322,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
               else if (geo.mode == MODE_UP4) { x = tx0 + (tap % 3) - 1;     y = ty0 + (tap / 3) - 1; }      // tap = shift index
               else                           { x = tx0 + px - (tap & 1);    y = ty0 + py - (tap >> 1); }
               tma_load_4d(s.a[st], &mapA, &s.full[st], ch, x, y, tn0);
-              tma_load_2d(s.b[st], &mapB, &s.full[st], kb * BK, n0 + (geo.mode == MODE_UP ? (int)blockIdx.z * geo.Cout : 0));
+              load_b_kmajor(st, kb * BK, n0 + (geo.mode == MODE_UP ? (int)blockIdx.z * geo.Cout : 0));
             }
           }
           __syncwarp();
         }
       }
-    } else {
+    } else if constexpr (!PRESPLIT) {
       // ===== B splitters: hi / lo halves of each landed B tile into the K-major swizzled operand buffers
       const int t = threadIdx.x - 32;
       int ntl = 0;
@@ -364,7 +395,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         const int st = it % STAGES;
         const uint32_t ph = (it / STAGES) & 1;
         mbar_wait(&s.full[st], ph);
-        mbar_wait(&s.split[st], ph);
+        if constexpr (!PRESPLIT) mbar_wait(&s.split[st], ph);
         // A fragment of the 4 k-steps (tf32 m64k8 layout: a0 (g, t), a1 (g+8, t), a2 (g, t+4), a3 (g+8, t+4))
         const char* araw = reinterpret_cast<const char*>(s.a[st]);
         uint32_t ahi[4][4], alo[4][4];
@@ -593,16 +624,55 @@ static unsigned persistent_grid_y(int tiles, unsigned gz) {
   return gy < (unsigned)tiles ? gy : (unsigned)tiles;
 }
 
-__global__ void conv_pack_down_kernel(const float* __restrict__ W, float* __restrict__ P, int Cs, int Cb) {
+// The TF32 split the B splitters apply in-kernel: hi = x with the 13 low mantissa bits cleared, lo = x - hi (exact)
+__device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
+// P[i] = v, or with a lo plane L: P[i] = hi(v), L[i] = v - hi(v)
+__device__ __forceinline__ void store_split(float* P, float* L, long long i, float v) {
+  if (L) { const float h = tf32_hi(v); P[i] = h; L[i] = v - h; }
+  else P[i] = v;
+}
+
+__global__ void tf32_split_kernel(const float* __restrict__ X, float* __restrict__ H, float* __restrict__ L, long long n) {
+  const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 4;
+  if (i + 4 <= n && !((reinterpret_cast<uintptr_t>(X) | reinterpret_cast<uintptr_t>(H) | reinterpret_cast<uintptr_t>(L)) & 15)) {
+    const float4 v = *reinterpret_cast<const float4*>(X + i);
+    const float4 h = make_float4(tf32_hi(v.x), tf32_hi(v.y), tf32_hi(v.z), tf32_hi(v.w));
+    *reinterpret_cast<float4*>(H + i) = h;
+    *reinterpret_cast<float4*>(L + i) = make_float4(v.x - h.x, v.y - h.y, v.z - h.z, v.w - h.w);
+  } else {
+    for (long long j = i; j < i + 4 && j < n; ++j) store_split(H, L, j, X[j]);
+  }
+}
+
+// H[c][r], L[c][r] = split(W[r][c]) for r < rows; columns [rows, ldt) of H and L are zero.  32 x 32 tiles through shared
+// memory, both sides coalesced.
+__global__ void tf32_split_t_kernel(const float* __restrict__ W, float* __restrict__ H, float* __restrict__ L, int rows,
+                                    int cols, long long ldw, long long ldt) {
+  __shared__ float t[32][33];
+  const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
+  for (int j = threadIdx.y; j < 32; j += blockDim.y) {
+    const int r = r0 + j, c = c0 + threadIdx.x;
+    t[j][threadIdx.x] = (r < rows && c < cols) ? W[(long long)r * ldw + c] : 0.f;
+  }
+  __syncthreads();
+  for (int j = threadIdx.y; j < 32; j += blockDim.y) {
+    const int c = c0 + j, r = r0 + threadIdx.x;
+    if (c < cols && r < ldt) store_split(H, L, (long long)c * ldt + r, t[threadIdx.x][j]);
+  }
+}
+
+__global__ void conv_pack_down_kernel(const float* __restrict__ W, float* __restrict__ P, float* __restrict__ L, int Cs,
+                                      int Cb) {
   // P[cs][tap][cb] = W[cs][cb][tap]
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)Cs * Cb * 16) return;
   const int cb = (int)(idx % Cb);
   const int tap = (int)((idx / Cb) % 16);
   const int cs = (int)(idx / ((long long)Cb * 16));
-  P[idx] = W[((long long)cs * Cb + cb) * 16 + tap];
+  store_split(P, L, idx, W[((long long)cs * Cb + cb) * 16 + tap]);
 }
-__global__ void conv_pack_up_kernel(const float* __restrict__ W, float* __restrict__ P, int Cs, int Cb) {
+__global__ void conv_pack_up_kernel(const float* __restrict__ W, float* __restrict__ P, float* __restrict__ L, int Cs,
+                                    int Cb) {
   // P[parity][cb][t][cs] = W[cs][cb][ky][kx], ky = (1-py)+2j, kx = (1-px)+2i, t = 2j+i
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= (long long)Cs * Cb * 16) return;
@@ -612,10 +682,11 @@ __global__ void conv_pack_up_kernel(const float* __restrict__ W, float* __restri
   const int par = (int)(idx / ((long long)Cs * 4 * Cb));
   const int py = par >> 1, px = par & 1;
   const int ky = (1 - py) + 2 * (t >> 1), kx = (1 - px) + 2 * (t & 1);
-  P[idx] = W[((long long)cs * Cb + cb) * 16 + ky * 4 + kx];
+  store_split(P, L, idx, W[((long long)cs * Cb + cb) * 16 + ky * 4 + kx]);
 }
 
-__global__ void conv_pack_up4_kernel(const float* __restrict__ W, float* __restrict__ P, int Cs, int Cb) {
+__global__ void conv_pack_up4_kernel(const float* __restrict__ W, float* __restrict__ P, float* __restrict__ L, int Cs,
+                                     int Cb) {
   // P[parity * Cb + cb][shift * Cs + cs] = W[cs][cb][ky][kx] when output parity (py, px) reads shift (dy, dx) (j = py - dy,
   // i = px - dx in {0, 1}; ky = (1 - py) + 2j, kx = (1 - px) + 2i), else 0.  shift = (dy + 1) * 3 + (dx + 1).
   const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -628,7 +699,7 @@ __global__ void conv_pack_up4_kernel(const float* __restrict__ W, float* __restr
   const int j = py - dy, i = px - dx;
   float v = 0.f;
   if (j >= 0 && j <= 1 && i >= 0 && i <= 1) v = W[((long long)cs * Cb + cb) * 16 + ((1 - py) + 2 * j) * 4 + (1 - px) + 2 * i];
-  P[idx] = v;
+  store_split(P, L, idx, v);
 }
 static bool conv_up_merged(int Cb) { return Cb == 32; }
 
@@ -700,26 +771,35 @@ splitk_reduce_kernel(const float* __restrict__ part, float* __restrict__ C, cons
   }
 }
 
-// one launch site for the four instantiations (tile width x TF32 passes)
-#define LAUNCH_GEMM_TC(BN_, PASSES_, grid_, st_, ...)                                                                \
+// one launch site for the eight instantiations (tile width x TF32 passes x B source)
+#define LAUNCH_GEMM_TC(BN_, PASSES_, PRE_, grid_, st_, ...)                                                          \
   do {                                                                                                               \
-    const size_t smem__ = sizeof(Smem<BN_>) + 1024;                                                                  \
-    RL_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN_, PASSES_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem__)); \
-    gemm_tc_kernel<BN_, PASSES_><<<grid_, NTHREADS, smem__, st_>>>(__VA_ARGS__);                                      \
+    static_assert(sizeof(Smem<BN_, PASSES_, PRE_>) + 1024 <= 227 * 1024, "operand stages exceed shared memory");     \
+    const size_t smem__ = sizeof(Smem<BN_, PASSES_, PRE_>) + 1024;                                                   \
+    RL_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN_, PASSES_, PRE_>, cudaFuncAttributeMaxDynamicSharedMemorySize,     \
+                                 (int)smem__));                                                                      \
+    gemm_tc_kernel<BN_, PASSES_, PRE_><<<grid_, NTHREADS, smem__, st_>>>(__VA_ARGS__);                                \
   } while (0)
-#define DISPATCH_GEMM_TC(BN_val, passes_val, grid_, st_, ...)                                  \
+#define DISPATCH_GEMM_TC_PRE(BN_val, passes_val, PRE_, grid_, st_, ...)                        \
   do {                                                                                          \
     if ((BN_val) == 64) {                                                                       \
-      if ((passes_val) == 3) LAUNCH_GEMM_TC(64, 3, grid_, st_, __VA_ARGS__);                    \
-      else LAUNCH_GEMM_TC(64, 1, grid_, st_, __VA_ARGS__);                                      \
+      if ((passes_val) == 3) LAUNCH_GEMM_TC(64, 3, PRE_, grid_, st_, __VA_ARGS__);              \
+      else LAUNCH_GEMM_TC(64, 1, PRE_, grid_, st_, __VA_ARGS__);                                \
     } else {                                                                                    \
-      if ((passes_val) == 3) LAUNCH_GEMM_TC(128, 3, grid_, st_, __VA_ARGS__);                   \
-      else LAUNCH_GEMM_TC(128, 1, grid_, st_, __VA_ARGS__);                                     \
+      if ((passes_val) == 3) LAUNCH_GEMM_TC(128, 3, PRE_, grid_, st_, __VA_ARGS__);             \
+      else LAUNCH_GEMM_TC(128, 1, PRE_, grid_, st_, __VA_ARGS__);                               \
     }                                                                                           \
   } while (0)
+// mb2: the lo plane's map when `presplit`, else ignored
+#define DISPATCH_GEMM_TC(BN_val, passes_val, presplit_, grid_, st_, ma_, mb_, mb2_, ...)                    \
+  do {                                                                                                       \
+    if (presplit_) DISPATCH_GEMM_TC_PRE(BN_val, passes_val, true, grid_, st_, ma_, mb_, mb2_, __VA_ARGS__);  \
+    else DISPATCH_GEMM_TC_PRE(BN_val, passes_val, false, grid_, st_, ma_, mb_, mb_, __VA_ARGS__);           \
+  } while (0)
 
-int launch_conv(int mode, const float* img, const float* Wp, float* out, const float* bias, int NB, int h, int w, int Cin,
-                int Cout, cudaStream_t st) {
+// Wp: the packed weight; Wlo: its TF32 lo plane when Wp holds the hi plane (pre-split B), else null
+int launch_conv(int mode, const float* img, const float* Wp, const float* Wlo, float* out, const float* bias, int NB, int h,
+                int w, int Cin, int Cout, cudaStream_t st) {
   TileGeo g = {};
   g.mode = mode; g.h = h; g.w = w; g.NB = NB; g.chunks = Cin / BK; g.Cout = Cout; g.ksplits = 1;
   g.passes = g_passes;
@@ -734,13 +814,15 @@ int launch_conv(int mode, const float* img, const float* Wp, float* out, const f
   const int BN = (mode == MODE_UP4) ? 128 : ((Cout <= 64) ? 64 : 128);
   const int brows = (mode == MODE_UP || mode == MODE_UP4) ? 4 * Cout : Cout;
   if (int rc = get_map(Wp, brows, K, K, BN, &mb)) return rc;
+  CUtensorMap mb2 = mb;
+  if (Wlo && g.passes == 3) { if (int rc = get_map(Wlo, brows, K, K, BN, &mb2)) return rc; }
   const int mtiles = g.tiles_x * g.tiles_y * (NB / g.bn);
   g.mtiles = mtiles;
   g.ntiles = (mode == MODE_UP4) ? 1 : (Cout + BN - 1) / BN;
   dim3 grid(1, 1, mode == MODE_UP ? 4 : 1);
   grid.y = persistent_grid_y(mtiles * g.ntiles, grid.z);
   const int M = NB * h * w;  // unused by conv addressing; row validity comes from geo
-  DISPATCH_GEMM_TC(BN, g.passes, grid, st, ma, mb, out, bias, M, Cout, K, Cout, 0, g);
+  DISPATCH_GEMM_TC(BN, g.passes, Wlo != nullptr, grid, st, ma, mb, mb2, out, bias, M, Cout, K, Cout, 0, g);
   RL_CHECK_LAUNCH();
   return B200RL_OK;
 }
@@ -766,26 +848,65 @@ extern "C" int b200rl_conv_tc_supported(int mode_up, int NB, int h, int w, int C
   if (Cin % BK != 0 || Cout < 16 || Cout % 4 != 0) return 0;
   return 1;
 }
-extern "C" int b200rl_conv_pack(const float* W, float* Wpacked, int mode_up, int Cs, int Cb, cudaStream_t st) {
-  RL_CHECK_ARG(W && Wpacked, "null pointer");
+namespace {
+int conv_pack_impl(const float* W, float* P, float* L, int mode_up, int Cs, int Cb, cudaStream_t st) {
   const long long n = (long long)Cs * Cb * 16;
-  if (mode_up && conv_up_merged(Cb)) conv_pack_up4_kernel<<<ceil_div(36LL * Cs * Cb, 256), 256, 0, st>>>(W, Wpacked, Cs, Cb);
-  else if (mode_up) conv_pack_up_kernel<<<ceil_div(n, 256), 256, 0, st>>>(W, Wpacked, Cs, Cb);
-  else conv_pack_down_kernel<<<ceil_div(n, 256), 256, 0, st>>>(W, Wpacked, Cs, Cb);
+  if (mode_up && conv_up_merged(Cb)) conv_pack_up4_kernel<<<ceil_div(36LL * Cs * Cb, 256), 256, 0, st>>>(W, P, L, Cs, Cb);
+  else if (mode_up) conv_pack_up_kernel<<<ceil_div(n, 256), 256, 0, st>>>(W, P, L, Cs, Cb);
+  else conv_pack_down_kernel<<<ceil_div(n, 256), 256, 0, st>>>(W, P, L, Cs, Cb);
   RL_CHECK_LAUNCH();
   return B200RL_OK;
+}
+}  // namespace
+extern "C" int b200rl_conv_pack(const float* W, float* Wpacked, int mode_up, int Cs, int Cb, cudaStream_t st) {
+  RL_CHECK_ARG(W && Wpacked, "null pointer");
+  return conv_pack_impl(W, Wpacked, nullptr, mode_up, Cs, Cb, st);
+}
+extern "C" int b200rl_conv_pack_split(const float* W, float* Whi, float* Wlo, int mode_up, int Cs, int Cb, cudaStream_t st) {
+  RL_CHECK_ARG(W && Whi && Wlo, "null pointer");
+  return conv_pack_impl(W, Whi, Wlo, mode_up, Cs, Cb, st);
 }
 extern "C" int b200rl_conv_down_tc(const float* big, const float* Wpacked, float* small_, int NB, int h, int w, int Cs,
                                    int Cb, cudaStream_t st) {
   RL_CHECK_ARG(big && Wpacked && small_, "null pointer");
   RL_CHECK_ARG(b200rl_conv_tc_supported(0, NB, h, w, Cs, Cb), "shape not eligible for the tensor-core conv path");
-  return launch_conv(MODE_DOWN, big, Wpacked, small_, nullptr, NB, h, w, Cb, Cs, st);
+  return launch_conv(MODE_DOWN, big, Wpacked, nullptr, small_, nullptr, NB, h, w, Cb, Cs, st);
 }
 extern "C" int b200rl_conv_up_tc(const float* small_, const float* Wpacked, float* big, const float* bias, int NB, int h,
                                  int w, int Cs, int Cb, cudaStream_t st) {
   RL_CHECK_ARG(big && Wpacked && small_, "null pointer");
   RL_CHECK_ARG(b200rl_conv_tc_supported(1, NB, h, w, Cs, Cb), "shape not eligible for the tensor-core conv path");
-  return launch_conv(MODE_UP, small_, Wpacked, big, bias, NB, h, w, Cs, Cb, st);
+  return launch_conv(MODE_UP, small_, Wpacked, nullptr, big, bias, NB, h, w, Cs, Cb, st);
+}
+extern "C" int b200rl_conv_down_tc_presplit(const float* big, const float* Whi, const float* Wlo, float* small_, int NB,
+                                            int h, int w, int Cs, int Cb, cudaStream_t st) {
+  RL_CHECK_ARG(big && Whi && Wlo && small_, "null pointer");
+  RL_CHECK_ARG(b200rl_conv_tc_supported(0, NB, h, w, Cs, Cb), "shape not eligible for the tensor-core conv path");
+  return launch_conv(MODE_DOWN, big, Whi, Wlo, small_, nullptr, NB, h, w, Cb, Cs, st);
+}
+extern "C" int b200rl_conv_up_tc_presplit(const float* small_, const float* Whi, const float* Wlo, float* big,
+                                          const float* bias, int NB, int h, int w, int Cs, int Cb, cudaStream_t st) {
+  RL_CHECK_ARG(big && Whi && Wlo && small_, "null pointer");
+  RL_CHECK_ARG(b200rl_conv_tc_supported(1, NB, h, w, Cs, Cb), "shape not eligible for the tensor-core conv path");
+  return launch_conv(MODE_UP, small_, Whi, Wlo, big, bias, NB, h, w, Cs, Cb, st);
+}
+
+extern "C" int b200rl_tf32_split(const float* X, float* Xhi, float* Xlo, long long n, cudaStream_t st) {
+  RL_CHECK_ARG(X && Xhi && Xlo, "null pointer");
+  RL_CHECK_ARG(n >= 0, "negative length");
+  if (n == 0) return B200RL_OK;
+  tf32_split_kernel<<<ceil_div((n + 3) / 4, 256), 256, 0, st>>>(X, Xhi, Xlo, n);
+  RL_CHECK_LAUNCH();
+  return B200RL_OK;
+}
+extern "C" int b200rl_tf32_split_t(const float* W, float* Thi, float* Tlo, int rows, int cols, long long ldw, long long ldt,
+                                   cudaStream_t st) {
+  RL_CHECK_ARG(W && Thi && Tlo, "null pointer");
+  RL_CHECK_ARG(rows > 0 && cols > 0 && ldw >= cols && ldt >= rows, "bad transposed-split geometry");
+  dim3 grid(ceil_div(cols, 32), ceil_div(ldt, 32));
+  tf32_split_t_kernel<<<grid, dim3(32, 8), 0, st>>>(W, Thi, Tlo, rows, cols, ldw, ldt);
+  RL_CHECK_LAUNCH();
+  return B200RL_OK;
 }
 
 // Shapes the tensor-core path accepts: NT product, 16-byte aligned operands with row strides that are
@@ -808,17 +929,22 @@ namespace {
 // workspace geometry.
 struct FusedTail { float* part; int ks, mpad, ldw; };
 
-int gemm_tc_impl(const float* A, const float* B, float* C, const float* bias, int M, int N, int K, int lda,
-                 int ldb, int ldc, int transA, int transB, int accumulate, cudaStream_t st, FusedTail* fused) {
+// Blo: non-null when B is given as its TF32 planes, B = hi plane and Blo = lo plane, both [N][K] (transB) with row
+// stride ldb
+int gemm_tc_impl(const float* A, const float* B, const float* Blo, float* C, const float* bias, int M, int N, int K,
+                 int lda, int ldb, int ldc, int transA, int transB, int accumulate, cudaStream_t st, FusedTail* fused) {
   RL_CHECK_ARG(A && B && (C || fused), "null pointer");
   RL_CHECK_ARG(b200rl_gemm_tc_supported(A, B, M, N, K, lda, ldb, transA, transB), "shape not eligible for the tensor-core path");
+  RL_CHECK_ARG(!Blo || (transB && !(reinterpret_cast<uintptr_t>(Blo) & 15)), "pre-split B must be 16-byte aligned [N][K] planes");
   const int BN = (N <= 64) ? 64 : 128;
-  CUtensorMap ma, mb;
+  CUtensorMap ma, mb, mb2;
   // A: [M][K] (K-major) or, transposed, [K][M] (MN-major: boxes of 32 k-rows x 32 m);  B: [N][K] or [K][N]
   if (!transA) { if (int rc = get_map(A, M, K, lda, BM, &ma)) return rc; }
   else         { if (int rc = get_map(A, K, M, lda, 32, &ma)) return rc; }
   if (transB)  { if (int rc = get_map(B, N, K, ldb, BN, &mb)) return rc; }
   else         { if (int rc = get_map(B, K, N, ldb, 32, &mb)) return rc; }
+  mb2 = mb;
+  if (Blo && g_passes == 3) { if (int rc = get_map(Blo, N, K, ldb, BN, &mb2)) return rc; }
   dim3 grid((N + BN - 1) / BN, (M + BM - 1) / BM);
   TileGeo g = {};
   g.mode = MODE_GEMM;
@@ -854,7 +980,7 @@ int gemm_tc_impl(const float* A, const float* B, float* C, const float* bias, in
   g.ntiles = (int)grid.x;
   grid.x = 1;
   grid.y = persistent_grid_y(g.mtiles * g.ntiles, grid.z);
-  DISPATCH_GEMM_TC(BN, g.passes, grid, st, ma, mb, C, bias, M, N, K, ldc, accumulate, g);
+  DISPATCH_GEMM_TC(BN, g.passes, Blo != nullptr, grid, st, ma, mb, mb2, C, bias, M, N, K, ldc, accumulate, g);
   RL_CHECK_LAUNCH();
   if (g.ksplits > 1 && !fused) {
     splitk_reduce_kernel<<<ceil_div((long long)M * ((N + 3) / 4), 256), 256, 0, st>>>(g.part, C, bias, M, N, ldc, g.ksplits, g.mpad,
@@ -949,7 +1075,17 @@ splitk_ln_kernel(const float* __restrict__ part, int ks, int mpad, int ldw, int 
 
 extern "C" int b200rl_gemm_tc(const float* A, const float* B, float* C, const float* bias, int M, int N, int K, int lda,
                               int ldb, int ldc, int transA, int transB, int accumulate, cudaStream_t st) {
-  return gemm_tc_impl(A, B, C, bias, M, N, K, lda, ldb, ldc, transA, transB, accumulate, st, nullptr);
+  return gemm_tc_impl(A, B, nullptr, C, bias, M, N, K, lda, ldb, ldc, transA, transB, accumulate, st, nullptr);
+}
+
+extern "C" int b200rl_gemm_tc_presplit_supported(const float* A, const float* Bhi, const float* Blo, int M, int N, int K,
+                                                 int lda, int ldb) {
+  return b200rl_gemm_tc_supported(A, Bhi, M, N, K, lda, ldb, 0, 1) && !(reinterpret_cast<uintptr_t>(Blo) & 15);
+}
+extern "C" int b200rl_gemm_tc_presplit(const float* A, const float* Bhi, const float* Blo, float* C, const float* bias, int M,
+                                       int N, int K, int lda, int ldb, int ldc, int accumulate, cudaStream_t st) {
+  RL_CHECK_ARG(Blo, "null pointer");
+  return gemm_tc_impl(A, Bhi, Blo, C, bias, M, N, K, lda, ldb, ldc, 0, 1, accumulate, st, nullptr);
 }
 
 extern "C" int b200rl_gemm_ln_supported(const float* A, const float* B, int M, int N, int K, int lda, int ldb, int mode) {
@@ -959,10 +1095,12 @@ extern "C" int b200rl_gemm_ln_supported(const float* A, const float* B, int M, i
   return 1;
 }
 
-extern "C" int b200rl_gemm_ln(const float* A, const float* W, int M, int N, int K, int lda, int ldw_, const float* gamma,
-                              const float* beta, float eps, int act, float* pre, long long ldpre, float* out, long long ldout,
-                              int mode, const float* h_prev, long long ldh, float* h_out, long long ldho, float* h_out2,
-                              long long ldho2, cudaStream_t st) {
+namespace {
+// Wlo: non-null when W is the TF32 hi plane of the weight and Wlo its lo plane
+int gemm_ln_impl(const float* A, const float* W, const float* Wlo, int M, int N, int K, int lda, int ldw_, const float* gamma,
+                 const float* beta, float eps, int act, float* pre, long long ldpre, float* out, long long ldout, int mode,
+                 const float* h_prev, long long ldh, float* h_out, long long ldho, float* h_out2, long long ldho2,
+                 cudaStream_t st) {
   RL_CHECK_ARG(A && W && gamma && beta, "null pointer");
   RL_CHECK_ARG(b200rl_gemm_ln_supported(A, W, M, N, K, lda, ldw_, mode), "shape not eligible for the fused product + LayerNorm");
   RL_CHECK_ARG(mode == 0 ? out != nullptr : (h_prev && h_out), "missing output");
@@ -972,7 +1110,7 @@ extern "C" int b200rl_gemm_ln(const float* A, const float* W, int M, int N, int 
                    ((ldpre | ldout | ldh | ldho | ldho2) & 3) == 0,
                "fused product + LayerNorm needs 16-byte aligned rows");
   FusedTail ft;
-  if (int rc = gemm_tc_impl(A, W, nullptr, nullptr, M, N, K, lda, ldw_, N, 0, 1, 0, st, &ft)) return rc;
+  if (int rc = gemm_tc_impl(A, W, Wlo, nullptr, nullptr, M, N, K, lda, ldw_, N, 0, 1, 0, st, &ft)) return rc;
   const int blocks = ceil_div((long long)M * 32, 256);
 #define LAUNCH_SPLITK_LN(NV_)                                                                                              \
   splitk_ln_kernel<NV_><<<blocks, 256, 0, st>>>(ft.part, ft.ks, ft.mpad, ft.ldw, M, N, gamma, beta, eps, act, pre, ldpre, out, \
@@ -988,6 +1126,28 @@ extern "C" int b200rl_gemm_ln(const float* A, const float* W, int M, int N, int 
 #undef LAUNCH_SPLITK_LN
   RL_CHECK_LAUNCH();
   return B200RL_OK;
+}
+}  // namespace
+
+extern "C" int b200rl_gemm_ln(const float* A, const float* W, int M, int N, int K, int lda, int ldw_, const float* gamma,
+                              const float* beta, float eps, int act, float* pre, long long ldpre, float* out, long long ldout,
+                              int mode, const float* h_prev, long long ldh, float* h_out, long long ldho, float* h_out2,
+                              long long ldho2, cudaStream_t st) {
+  return gemm_ln_impl(A, W, nullptr, M, N, K, lda, ldw_, gamma, beta, eps, act, pre, ldpre, out, ldout, mode, h_prev, ldh,
+                      h_out, ldho, h_out2, ldho2, st);
+}
+extern "C" int b200rl_gemm_ln_presplit_supported(const float* A, const float* Whi, const float* Wlo, int M, int N, int K,
+                                                 int lda, int ldw, int mode) {
+  return b200rl_gemm_ln_supported(A, Whi, M, N, K, lda, ldw, mode) && !(reinterpret_cast<uintptr_t>(Wlo) & 15);
+}
+extern "C" int b200rl_gemm_ln_presplit(const float* A, const float* Whi, const float* Wlo, int M, int N, int K, int lda,
+                                       int ldw, const float* gamma, const float* beta, float eps, int act, float* pre,
+                                       long long ldpre, float* out, long long ldout, int mode, const float* h_prev,
+                                       long long ldh, float* h_out, long long ldho, float* h_out2, long long ldho2,
+                                       cudaStream_t st) {
+  RL_CHECK_ARG(Wlo, "null pointer");
+  return gemm_ln_impl(A, Whi, Wlo, M, N, K, lda, ldw, gamma, beta, eps, act, pre, ldpre, out, ldout, mode, h_prev, ldh,
+                      h_out, ldho, h_out2, ldho2, st);
 }
 
 // ---- convolution weight gradient on the tensor cores, operands read in place (no im2col, no transposes):
@@ -1032,7 +1192,7 @@ extern "C" int b200rl_conv_wgrad_mn(const float* small_, const float* big, float
   }
   grid.x = 1;
   grid.y = (unsigned)(g.mtiles * g.ntiles);
-  DISPATCH_GEMM_TC(BN, g.passes, grid, st, ma, mb, G, nullptr, M, N, P, N, 0, g);
+  DISPATCH_GEMM_TC(BN, g.passes, false, grid, st, ma, mb, mb, G, nullptr, M, N, P, N, 0, g);
   RL_CHECK_LAUNCH();
   if (g.ksplits > 1) {
     splitk_reduce_kernel<<<ceil_div((long long)M * ((N + 3) / 4), 256), 256, 0, st>>>(g.part, G, nullptr, M, N, N, g.ksplits, g.mpad,

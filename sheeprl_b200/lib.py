@@ -19,6 +19,11 @@ HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "b200rl.h")
 
 _lib = None
 
+# Tensor-core products with at least this many rows take B as pre-split TF32 planes: one streaming split pass over B
+# (12 bytes per element) in place of the kernel splitting the B tile again in every one of the M / 128 row tiles.  At
+# 32 row tiles and more the pass costs a small fraction of what it saves (DESIGN.md §4, "Pre-split weight operands").
+PRESPLIT_MIN_ROWS = 4096
+
 
 class B200RLError(RuntimeError):
     pass
@@ -181,9 +186,29 @@ class CudaOps:
         assert (A.shape[1] if transA else A.shape[0]) == M, (A.shape, C.shape, transA)
         assert (B.shape[0] if transB else B.shape[1]) == N and (B.shape[1] if transB else B.shape[0]) == K, \
             (A.shape, B.shape, C.shape, transA, transB)
+        if (not transA and M >= PRESPLIT_MIN_ROWS and self.use_tc
+                and self.lib.b200rl_gemm_tc_supported(_p(A), _p(B), M, N, K, _ld(A), _ld(B), 0, int(transB))):
+            hi, lo, ld = self._planes(B, transB, N, K)
+            self._ck(self.lib.b200rl_gemm_tc_presplit(_p(A), _p(hi), _p(lo), _p(C), _p(bias), M, N, K, _ld(A), ld, _ld(C),
+                                                      int(accumulate), self._st()))
+            return
         # every layout goes to one entry point: transposed operands are read in place as MN-major tiles
         self._ck(self.lib.b200rl_gemm_f32(_p(A), _p(B), _p(C), _p(bias), M, N, K, _ld(A), _ld(B), _ld(C), int(transA),
                                           int(transB), int(accumulate), self._st()))
+
+    def _planes(self, B, transB: bool, N: int, K: int):
+        """(hi, lo, ld): B as the K-major [N][K] TF32 planes (row stride ld) of b200rl_gemm_tc_presplit, in a workspace
+        reused by consecutive products on the stream.  A [N][K] B keeps its row stride (the split runs over the whole
+        strided span); a [K][N] B is split transposed, rows padded to a multiple of 4 floats."""
+        ldb = _ld(B)
+        ld = ldb if transB else (K + 3) // 4 * 4
+        buf = self._scratch("b_planes", 2 * N * ld)
+        hi, lo = buf[:N * ld], buf[N * ld:2 * N * ld]
+        if transB:
+            self._ck(self.lib.b200rl_tf32_split(_p(B), _p(hi), _p(lo), (N - 1) * ldb + K, self._st()))
+        else:
+            self._ck(self.lib.b200rl_tf32_split_t(_p(B), _p(hi), _p(lo), K, N, ldb, ld, self._st()))
+        return hi, lo, ld
 
     def gemm_ln_supported(self, A, W, mode: int = 0) -> bool:
         M, K = A.shape
@@ -251,22 +276,24 @@ class CudaOps:
         Cb = big.shape[-1]
         assert tuple(big.shape) == (NB, 2 * h, 2 * w, Cb) and tuple(W.shape) == (Cs, Cb, 4, 4)
         if self.use_tc and self.lib.b200rl_conv_tc_supported(0, NB, h, w, Cs, Cb):
-            Wp = self._packed(W, 0, Cs, Cb)
-            self._ck(self.lib.b200rl_conv_down_tc(_p(big), _p(Wp), _p(small), NB, h, w, Cs, Cb, self._st()))
+            hi, lo = self._packed(W, 0, Cs, Cb)
+            self._ck(self.lib.b200rl_conv_down_tc_presplit(_p(big), _p(hi), _p(lo), _p(small), NB, h, w, Cs, Cb,
+                                                           self._st()))
             return
         self._ck(self.lib.b200rl_conv_down(_p(big), _p(W), _p(small), NB, h, w, Cs, Cb, self._st()))
 
     def _packed(self, W, mode_up: int, Cs: int, Cb: int):
-        """Tap-major copy of a conv weight for the tensor-core kernels (caller-owned workspace, refreshed on every
-        use because the optimiser rewrites W each step; 16*Cs*Cb floats, a few microseconds)."""
+        """Tap-major copy of a conv weight for the tensor-core kernels as its TF32 hi / lo planes (caller-owned
+        workspace, refreshed on every use because the optimiser rewrites W each step; 2 x 16*Cs*Cb floats, a few
+        microseconds).  The split here spares the kernel splitting the weight tile again for every output tile."""
         key = (W.data_ptr(), mode_up)
         buf = self._pack_bufs.get(key)
         need = self.lib.b200rl_conv_pack_floats(mode_up, Cs, Cb)
-        if buf is None or buf.numel() != need:
-            buf = torch.empty(need, dtype=torch.float32, device=W.device)
+        if buf is None or buf.shape != (2, need):
+            buf = torch.empty(2, need, dtype=torch.float32, device=W.device)
             self._pack_bufs[key] = buf
-        self._ck(self.lib.b200rl_conv_pack(_p(W), _p(buf), mode_up, Cs, Cb, self._st()))
-        return buf
+        self._ck(self.lib.b200rl_conv_pack_split(_p(W), _p(buf[0]), _p(buf[1]), mode_up, Cs, Cb, self._st()))
+        return buf[0], buf[1]
 
     def conv_up(self, small, W, big, bias=None):
         _f32(big, W, small, bias)
@@ -275,8 +302,9 @@ class CudaOps:
         Cb = big.shape[-1]
         assert tuple(big.shape) == (NB, 2 * h, 2 * w, Cb) and tuple(W.shape) == (Cs, Cb, 4, 4)
         if self.use_tc and self.lib.b200rl_conv_tc_supported(1, NB, h, w, Cs, Cb):
-            Wp = self._packed(W, 1, Cs, Cb)
-            self._ck(self.lib.b200rl_conv_up_tc(_p(small), _p(Wp), _p(big), _p(bias), NB, h, w, Cs, Cb, self._st()))
+            hi, lo = self._packed(W, 1, Cs, Cb)
+            self._ck(self.lib.b200rl_conv_up_tc_presplit(_p(small), _p(hi), _p(lo), _p(big), _p(bias), NB, h, w, Cs, Cb,
+                                                         self._st()))
             return
         self._ck(self.lib.b200rl_conv_up(_p(small), _p(W), _p(big), _p(bias), NB, h, w, Cs, Cb, self._st()))
 

@@ -11,7 +11,7 @@ import torch
 from sheeprl_b200.lib import CudaOps
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from gemm_bench import SHAPES  # noqa: E402
+from gemm_bench import SHAPES, gemm_presplit, planes  # noqa: E402
 
 CONV_LAYERS = ((1024, 16, 64, 32), (1024, 8, 128, 64), (1024, 4, 256, 128))   # NB, h, Cs, Cb (tensor-core eligible)
 
@@ -40,7 +40,12 @@ def main():
             B = draw((N, K) if tB else (K, N), 100 * i + 2)
             C = torch.empty(M, N, device="cuda")
             cu.gemm(A, B, C, tA, tB)
-            out[f"{prec}/gemm_M{M}_N{N}_K{K}_{'T' if tA else 'N'}{'T' if tB else 'N'}"] = digest(C)
+            tag = f"{prec}/gemm_M{M}_N{N}_K{K}_{'T' if tA else 'N'}{'T' if tB else 'N'}"
+            out[tag] = digest(C)
+            if not tA:              # B as pre-split TF32 planes: must give the raw-B bits
+                C.fill_(float("nan"))
+                gemm_presplit(cu, A, planes(cu, B, tB), C)
+                out[tag + "_presplit"] = digest(C)
             del A, B, C
         # the imagination tails: product + LayerNorm + SiLU, product + LayerNorm + GRU gate
         M, N, K = 1024, 512, 1536
@@ -68,13 +73,19 @@ def main():
     cu.set_matmul_precision("highest")
     json.dump(out, open(a.json, "w"), indent=1, sort_keys=True)
     print(f"{len(out)} outputs hashed -> {a.json}")
+    routes = sorted(k for k in out if k.endswith("_presplit") and out[k] != out[k[: -len("_presplit")]])
+    for k in routes:
+        print(f"PRE-SPLIT DIFFERS FROM RAW B: {k}")
     if a.compare:
         ref = json.load(open(a.compare))
-        diff = sorted(k for k in set(ref) | set(out) if ref.get(k) != out.get(k))
+        both = set(ref) & set(out)
+        diff = sorted(k for k in both if ref[k] != out[k])
         for k in diff:
             print(f"DIFFERS: {k}")
-        print(f"{len(out) - len(diff)} / {len(set(ref) | set(out))} outputs bit-identical to {a.compare}")
-        sys.exit(1 if diff else 0)
+        print(f"{len(both) - len(diff)} / {len(both)} outputs both builds hash bit-identical to {a.compare}"
+              f" ({len(set(ref) ^ set(out))} routes hashed by one build only)")
+        sys.exit(1 if diff or routes else 0)
+    sys.exit(1 if routes else 0)
 
 
 if __name__ == "__main__":
