@@ -17,15 +17,15 @@ Layout decisions:
 from __future__ import annotations
 
 from collections import OrderedDict
-from typing import Dict, List, Optional, Sequence
+from typing import Dict, Optional, Sequence
 
 import torch
 
+from sheeprl_b200.dense import Act, LayerNormAct, Linear, Stack
 from sheeprl_b200.params import FlatGroup
 
 CONVS = ((8, 4, 32), (4, 2, 64), (3, 1, 64))        # NatureCNN (kernel, stride, channels) models.py:301-309
 LN_EPS = 1e-5                                        # nn.LayerNorm default (ppo/agent.py:63-64 passes only the shape)
-ACT_CODE = {"none": 0, "tanh": 2, "relu": 3}         # b200rl_ln_act_* activation codes
 DIST_MODE = {"discrete": 0, "normal": 1, "tanh_normal": 2}
 
 
@@ -36,41 +36,6 @@ def net_cfg(spec: dict, which: str):
     ln = spec.get("layer_norm", False)
     ln = bool(ln.get(which, False)) if isinstance(ln, dict) else bool(ln)
     return int(dense), int(layers), ln
-
-
-class _Lin:
-    """One Linear layer bound to flat-group views: W [1,out,in], b [1,out] and their gradients."""
-
-    def __init__(self, eng, wkey: str, act: str):
-        v, g = eng.group.views, eng.group.gviews
-        bkey = wkey[:-6] + "bias"
-        self.W, self.b = v[wkey].unsqueeze(0), v[bkey].unsqueeze(0)
-        self.gW, self.gb = g[wkey].unsqueeze(0), g[bkey].unsqueeze(0)
-        self.act = act
-        self.ln = None                                   # (gamma, beta, dgamma, dbeta) when a LayerNorm follows
-
-
-class _Stack:
-    """An `MLP` of the reference (models/models.py:17-126): `layers` hidden blocks Linear [-> LayerNorm] -> act, then an
-    output Linear without activation (absent for the actor backbone, whose output layer is the stacked action heads)."""
-
-    def __init__(self, eng, prefix: str, which: str, tag: str, last_key: Optional[str] = None):
-        dense, layers, ln = net_cfg(eng.spec, which)
-        st = 3 if ln else 2
-        v, g = eng.group.views, eng.group.gviews
-        self.tag, self.has_ln, self.dense = tag, ln, dense
-        self.lins: List[_Lin] = []
-        for i in range(layers):
-            lin = _Lin(eng, f"{prefix}._model.{st * i}.weight", eng.act)
-            if ln:
-                wk, bk = f"{prefix}._model.{st * i + 1}.weight", f"{prefix}._model.{st * i + 1}.bias"
-                lin.ln = (v[wk], v[bk], g[wk], g[bk])
-            self.lins.append(lin)
-        self.lins.append(_Lin(eng, last_key or f"{prefix}._model.{st * layers}.weight", "none"))
-
-    @property
-    def n_hidden(self):
-        return len(self.lins) - 1
 
 
 class PPOEngine:
@@ -109,6 +74,11 @@ class PPOEngine:
         self.losses = torch.zeros(3, dtype=torch.float32, device=self.device)
 
     # ------------------------------------------------------------------ parameters
+    @property
+    def actor_in(self) -> int:
+        """width of the actor's and critic's input: the features"""
+        return self.feat_dim
+
     def _internal_shapes(self):
         s, out = self.spec, OrderedDict()
         pre = "feature_extractor.cnn_encoder.model"
@@ -135,25 +105,33 @@ class PPOEngine:
 
         if s["mlp_dim"]:
             stack("feature_extractor.mlp_encoder.model", s["mlp_dim"], "encoder", s["mlp_features"])
-        stack("critic", self.feat_dim, "critic", 1)
-        stack("actor.actor_backbone", self.feat_dim, "actor", None)
+        stack("critic", self.actor_in, "critic", 1)
+        stack("actor.actor_backbone", self.actor_in, "actor", None)
         # every head reads `actor.dense_units` inputs, also with an empty backbone (ppo/agent.py:180-183)
         out["actor.heads.weight"] = (self.head_width, net_cfg(s, "actor")[0])
         out["actor.heads.bias"] = (self.head_width,)
         return out
 
     def _build_layers(self):
-        s = self.spec
         pre = "feature_extractor.cnn_encoder.model"
-        self.convs = [_Lin(self, f"{pre}._model.{2 * i}.weight", "relu") for i in range(len(self.geo))]
-        for c in self.convs:                              # [1, Cout, k*k*Cin]
-            c.W, c.gW = c.W.flatten(2), c.gW.flatten(2)
-        self.fc = _Lin(self, f"{pre}.fc.weight", "relu") if self.geo else None
-        self.menc = _Stack(self, "feature_extractor.mlp_encoder.model", "encoder", "m") if s["mlp_dim"] else None
-        self.critic = _Stack(self, "critic", "critic", "c")
-        self.actor = _Stack(self, "actor.actor_backbone", "actor", "a", last_key="actor.heads.weight")
-        if self.actor.n_hidden == 0 and self.actor.dense != self.feat_dim:
-            raise ValueError("actor.mlp_layers == 0 needs actor.dense_units == feature dim (the heads read dense_units inputs)")
+        self.convs = [Linear.of(self.group, f"{pre}._model.{2 * i}.weight") for i in range(len(self.geo))]
+        self.fc = Linear.of(self.group, f"{pre}.fc.weight") if self.geo else None
+        self.menc = self._stack("feature_extractor.mlp_encoder.model", "encoder") if self.spec["mlp_dim"] else None
+        self.critic = self._stack("critic", "critic")
+        self.actor = self._stack("actor.actor_backbone", "actor", last_key="actor.heads.weight")
+        if len(self.actor.layers) == 1 and net_cfg(self.spec, "actor")[0] != self.actor_in:
+            raise ValueError(f"actor.mlp_layers == 0 needs actor.dense_units == the actor's input width {self.actor_in} "
+                             "(the heads read dense_units inputs)")
+
+    def _stack(self, prefix: str, which: str, last_key: Optional[str] = None) -> Stack:
+        """An `MLP` of the reference (models/models.py:17-126): `layers` hidden blocks Linear [-> LayerNorm] -> act, then
+        an output Linear without activation (for the actor backbone: the stacked action heads)."""
+        _, layers, ln = net_cfg(self.spec, which)
+        st = 3 if ln else 2
+        out = [(Linear.of(self.group, f"{prefix}._model.{st * i}.weight"),
+                LayerNormAct(self.group, f"{prefix}._model.{st * i + 1}", LN_EPS, self.act) if ln else Act(self.act))
+               for i in range(layers)]
+        return Stack(self.ops, out + [(Linear.of(self.group, last_key or f"{prefix}._model.{st * layers}.weight"), Act("none"))])
 
     def reference_shapes(self) -> "OrderedDict[str, tuple]":
         out = OrderedDict()
@@ -235,57 +213,13 @@ class PPOEngine:
             b["dy"] = [f(1, B * Ho * Wo, Co) for (_, _, _, _, _, Ho, Wo, Co) in self.geo]
             b["dcol"] = [None] + [f(1, B * Ho * Wo, k * k * Ci) for (_, _, Ci, k, _, Ho, Wo, _) in self.geo[1:]]
         b["feat"], b["dfeat"] = f(1, B, self.feat_dim), f(1, B, self.feat_dim)
-        for st in (self.menc, self.critic, self.actor):
-            if st is None:
-                continue
-            n, D = st.n_hidden, st.dense
-            b[st.tag + "h"], b["d" + st.tag + "h"] = [f(1, B, D) for _ in range(n)], [f(1, B, D) for _ in range(n)]
-            b[st.tag + "pre"] = [f(1, B, D) for _ in range(n)] if st.has_ln else None     # pre-LayerNorm activations
+        for name, st in (("menc", self.menc), ("critic", self.critic), ("actor", self.actor)):
+            if st is not None:
+                b[name] = st.acts(B)
         b["values"], b["dvalues"] = f(1, B, 1), f(1, B, 1)
         b["head"], b["dhead"] = f(1, B, self.head_width), f(1, B, self.head_width)
         self._bufs[B] = b
         return b
-
-    # ------------------------------------------------------------------ layer helpers
-    def _fwd(self, lin: _Lin, x, y):
-        self.ops.bgemm(x, lin.W.transpose(1, 2), y, bias=lin.b, epi=lin.act)
-
-    def _bwd(self, lin: _Lin, dpre, x, dx=None, dx_epi="none", dx_aux=None, accumulate_dx=False, Wcols=None):
-        """weight/bias gradient of `lin` from the pre-activation gradient `dpre`; optionally the input gradient
-        (times the derivative `dx_epi` of the producer's activation, whose output is `dx_aux`)."""
-        o = self.ops
-        o.bgemm(dpre.transpose(1, 2), x, lin.gW, rsum=lin.gb)
-        if dx is not None:
-            W = lin.W if Wcols is None else lin.W[:, :, Wcols[0]:Wcols[1]]
-            o.bgemm(dpre, W, dx, aux=dx_aux, epi=dx_epi, accumulate=accumulate_dx)
-
-    def _mlp_fwd(self, st: _Stack, b: dict, x, out):
-        hidden, pre = b[st.tag + "h"], b[st.tag + "pre"]
-        for i, lin in enumerate(st.lins):
-            y = hidden[i] if i < st.n_hidden else out
-            if lin.ln is not None:                          # Linear -> LayerNorm -> act (utils/model.py:76-87)
-                self.ops.bgemm(x, lin.W.transpose(1, 2), pre[i], bias=lin.b)
-                self.ops.ln_act_fwd(pre[i][0], lin.ln[0], lin.ln[1], LN_EPS, ACT_CODE[lin.act], y[0])
-            else:
-                self._fwd(lin, x, y)
-            x = y
-
-    def _mlp_bwd(self, st: _Stack, b: dict, dout):
-        """backward through the stack down to its first layer; weight / LayerNorm gradients of layers >= 1 are written,
-        the return value is the gradient w.r.t. layer 0's Linear output (the caller owns layer 0's products)."""
-        hidden, dhidden, pre = b[st.tag + "h"], b["d" + st.tag + "h"], b[st.tag + "pre"]
-        dpre = dout
-        for i in range(st.n_hidden, 0, -1):
-            below = st.lins[i - 1]
-            if below.ln is not None:
-                self._bwd(st.lins[i], dpre, hidden[i - 1], dx=dhidden[i - 1])
-                gam, bet, dgam, dbet = below.ln
-                self.ops.ln_act_bwd(pre[i - 1][0], gam, bet, LN_EPS, ACT_CODE[below.act], dhidden[i - 1][0], dhidden[i - 1][0],
-                                    dgam, dbet)
-            else:
-                self._bwd(st.lins[i], dpre, hidden[i - 1], dx=dhidden[i - 1], dx_epi="d" + below.act, dx_aux=hidden[i - 1])
-            dpre = dhidden[i - 1]
-        return dpre
 
     def forward(self, b: dict, rgb, x_state, rgb_normalized: bool = False, actor: bool = True, critic: bool = True):
         """PPOAgent.forward up to the head / value outputs (ppo/agent.py:208-212) into the buffer set `b`.
@@ -303,15 +237,15 @@ class PPOEngine:
             x = b["x0"]
             for i, (H, W, C, k, st, Ho, Wo, Co) in enumerate(self.geo):
                 o.im2col(x, b["col"][i][0], k, st)
-                self._fwd(self.convs[i], b["col"][i], b["y"][i])
+                self.convs[i].forward(o, b["col"][i], b["y"][i], "relu")
                 x = b["y"][i][0].view(B, Ho, Wo, Co)
-            self._fwd(self.fc, b["y"][-1].view(1, B, -1), feat[:, :, :self.F])
+            self.fc.forward(o, b["y"][-1].view(1, B, -1), feat[:, :, :self.F], "relu")
         if self.menc is not None:
-            self._mlp_fwd(self.menc, b, x_state, feat[:, :, self.F:])
+            self.menc.forward(x_state, b["menc"], feat[:, :, self.F:])
         if critic:
-            self._mlp_fwd(self.critic, b, feat, b["values"])
+            self.critic.forward(feat, b["critic"], b["values"])
         if actor:
-            self._mlp_fwd(self.actor, b, feat, b["head"])
+            self.actor.forward(feat, b["actor"], b["head"])
 
     # ------------------------------------------------------------------ one minibatch
     def minibatch_step(self, data: Dict[str, torch.Tensor], idx: torch.Tensor):
@@ -341,16 +275,17 @@ class PPOEngine:
     def _backward(self, b: dict, x_state):
         """every weight gradient from b["dhead"] / b["dvalues"] (the objective's output) down to the encoders; each
         product reduces over all rows of `b`"""
-        o, F_, feat = self.ops, self.F, b["feat"]
         # actor, critic -> feature gradient (cnn columns masked by the fc ReLU)
-        for j, (st, dout) in enumerate(((self.actor, b["dhead"]), (self.critic, b["dvalues"]))):
-            dpre0, l0 = self._mlp_bwd(st, b, dout), st.lins[0]
-            o.bgemm(dpre0.transpose(1, 2), feat, l0.gW, rsum=l0.gb)
-            if F_:
-                o.bgemm(dpre0, l0.W[:, :, :F_], b["dfeat"][:, :, :F_], aux=feat[:, :, :F_], epi="drelu", accumulate=j > 0)
-            if self.Mf:
-                o.bgemm(dpre0, l0.W[:, :, F_:], b["dfeat"][:, :, F_:], accumulate=j > 0)
+        for j, (name, dout) in enumerate((("actor", b["dhead"]), ("critic", b["dvalues"]))):
+            getattr(self, name).backward(dout, b["feat"], b[name], self.feature_grads(b), accumulate=j > 0)
         self._encoder_bwd(b, x_state)
+
+    def feature_grads(self, b: dict, width: Optional[int] = None):
+        """`Linear.input_grad` products of the feature gradient b["dfeat"] from a layer whose first `width` (default:
+        all) inputs are the features: image columns times the fc ReLU's derivative, vector columns as they are"""
+        F_, feat, dfeat = self.F, b["feat"], b["dfeat"]
+        return ([(dfeat[:, :, :F_], slice(None, F_), "drelu", feat[:, :, :F_])] if F_ else []) + \
+               ([(dfeat[:, :, F_:], slice(F_, width), "none", None)] if self.Mf else [])
 
     def _encoder_bwd(self, b: dict, x_state):
         """weight gradients of the vector and image encoders from b["dfeat"] (its image columns already masked by the
@@ -358,19 +293,17 @@ class PPOEngine:
         o, F_ = self.ops, self.F
         B = b["dfeat"].shape[1]
         if self.menc is not None:
-            dpre0, l0 = self._mlp_bwd(self.menc, b, b["dfeat"][:, :, F_:]), self.menc.lins[0]
-            o.bgemm(dpre0.transpose(1, 2), x_state, l0.gW, rsum=l0.gb)
+            self.menc.backward(b["dfeat"][:, :, F_:], x_state, b["menc"])
         if self.geo:
-            n = len(self.geo)
             flat = b["y"][-1].view(1, B, -1)
-            self._bwd(self.fc, b["dfeat"][:, :, :F_], flat, dx=b["dy"][-1].view(1, B, -1), dx_epi="drelu", dx_aux=flat)
-            for i in range(n - 1, -1, -1):
+            self.fc.weight_grad(o, b["dfeat"][:, :, :F_], flat)
+            self.fc.input_grad(o, b["dfeat"][:, :, :F_], [(b["dy"][-1].view(1, B, -1), None, "drelu", flat)])
+            for i in range(len(self.geo) - 1, -1, -1):
                 H, W, C, k, st, Ho, Wo, Co = self.geo[i]
+                self.convs[i].weight_grad(o, b["dy"][i], b["col"][i])
                 if i > 0:
-                    self._bwd(self.convs[i], b["dy"][i], b["col"][i], dx=b["dcol"][i])
+                    self.convs[i].input_grad(o, b["dy"][i], [(b["dcol"][i], None, "none", None)])
                     o.col2im(b["dcol"][i][0], b["y"][i - 1][0].view(B, H, W, C), b["dy"][i - 1][0].view(B, H, W, C), k, st)
-                else:
-                    self._bwd(self.convs[0], b["dy"][0], b["col"][0])
 
     def _optimizer_step(self):
         o, hp = self.ops, self.hp

@@ -24,23 +24,10 @@ from typing import Dict, Optional, Sequence
 
 import torch
 
-from sheeprl_b200.algos.ppo.engine import ACT_CODE, PPOEngine, _Lin, _Stack
+from sheeprl_b200.algos.ppo.engine import PPOEngine
+from sheeprl_b200.dense import Act, LayerNormAct, Linear, Stack
 
 RNN_LN_EPS = 1e-3                                     # RecurrentModel's pre/post MLP LayerNorm (agent.py:31-35, 52-56)
-
-
-class _Dense:
-    """One hidden block Linear -> [LayerNorm(eps 1e-3)] -> act of the pre- / post-RNN MLP (models.py MLP with one
-    hidden size and no output layer): keys `{prefix}._model.0.*` and, with LayerNorm, `{prefix}._model.1.*`."""
-
-    def __init__(self, eng, prefix: str, ln: bool, act: str):
-        v, g = eng.group.views, eng.group.gviews
-        self.W, self.b = v[f"{prefix}._model.0.weight"].unsqueeze(0), v[f"{prefix}._model.0.bias"].unsqueeze(0)
-        self.gW, self.gb = g[f"{prefix}._model.0.weight"].unsqueeze(0), g[f"{prefix}._model.0.bias"].unsqueeze(0)
-        self.ln = (v[f"{prefix}._model.1.weight"], v[f"{prefix}._model.1.bias"], g[f"{prefix}._model.1.weight"],
-                   g[f"{prefix}._model.1.bias"]) if ln else None
-        self.act = act
-        self.dense = self.W.shape[1]
 
 
 class RecurrentPPOEngine(PPOEngine):
@@ -69,9 +56,14 @@ class RecurrentPPOEngine(PPOEngine):
     def lstm_in(self) -> int:
         return int(self.pre_cfg[0]) if self.pre_cfg else self.feat_dim + self.n_actions
 
+    @property
+    def actor_in(self) -> int:
+        """the critic and actor read the H-wide RNN output"""
+        return self.H
+
     def _internal_shapes(self):
         out = OrderedDict()
-        base = super()._internal_shapes()             # encoders, critic / actor on feat_dim inputs, stacked heads
+        base = super()._internal_shapes()             # encoders, critic / actor on H inputs, stacked heads
         for k, v in base.items():
             if k.startswith("feature_extractor."):
                 out[k] = v
@@ -89,31 +81,30 @@ class RecurrentPPOEngine(PPOEngine):
             out["rnn._post_mlp._model.0.weight"], out["rnn._post_mlp._model.0.bias"] = (H, H), (H,)
             if ln:
                 out["rnn._post_mlp._model.1.weight"], out["rnn._post_mlp._model.1.bias"] = (H,), (H,)
-        for k, v in base.items():                      # critic / actor read the H-wide RNN output
+        for k, v in base.items():
             if k.startswith(("critic.", "actor.")):
-                out[k] = (v[0], H) if k.endswith("._model.0.weight") else v
+                out[k] = v
         return out
 
     def _build_layers(self):
-        s = self.spec
-        pre = "feature_extractor.cnn_encoder.model"
-        self.convs = [_Lin(self, f"{pre}._model.{2 * i}.weight", "relu") for i in range(len(self.geo))]
-        for c in self.convs:
-            c.W, c.gW = c.W.flatten(2), c.gW.flatten(2)
-        self.fc = _Lin(self, f"{pre}.fc.weight", "relu") if self.geo else None
-        self.menc = _Stack(self, "feature_extractor.mlp_encoder.model", "encoder", "m") if s["mlp_dim"] else None
-        self.critic = _Stack(self, "critic", "critic", "c")
-        self.actor = _Stack(self, "actor.actor_backbone", "actor", "a", last_key="actor.heads.weight")
-        if self.actor.n_hidden == 0 and self.actor.dense != self.H:
-            raise ValueError("actor.mlp_layers == 0 needs actor.dense_units == rnn.lstm.hidden_size")
+        super()._build_layers()
         v, g = self.group.views, self.group.gviews
-        self.pre_mlp = _Dense(self, "rnn._pre_mlp", bool(self.pre_cfg[1]), self.act) if self.pre_cfg else None
-        self.post_mlp = _Dense(self, "rnn._post_mlp", bool(self.post_cfg[1]), self.act) if self.post_cfg else None
-        self.W_ih, self.gW_ih = v["rnn._lstm.weight_ih_l0"].unsqueeze(0), g["rnn._lstm.weight_ih_l0"].unsqueeze(0)
+        self.pre_mlp = self._rnn_mlp("rnn._pre_mlp", self.pre_cfg)
+        self.post_mlp = self._rnn_mlp("rnn._post_mlp", self.post_cfg)
+        self.bsum = torch.zeros(4 * self.H, dtype=torch.float32, device=self.device)    # b_ih + b_hh
+        self.W_ih = Linear(v["rnn._lstm.weight_ih_l0"].unsqueeze(0), self.bsum.unsqueeze(0),
+                           g["rnn._lstm.weight_ih_l0"].unsqueeze(0), g["rnn._lstm.bias_ih_l0"].unsqueeze(0))
         self.W_hh, self.gW_hh = v["rnn._lstm.weight_hh_l0"], g["rnn._lstm.weight_hh_l0"].unsqueeze(0)
         self.b_ih, self.b_hh = v["rnn._lstm.bias_ih_l0"], v["rnn._lstm.bias_hh_l0"]
         self.gb_ih, self.gb_hh = g["rnn._lstm.bias_ih_l0"], g["rnn._lstm.bias_hh_l0"]
-        self.bsum = torch.zeros(4 * self.H, dtype=torch.float32, device=self.device)
+
+    def _rnn_mlp(self, prefix: str, cfg) -> Optional[Stack]:
+        """the pre- / post-RNN MLP (models.py MLP with one hidden size and no output layer): Linear `{prefix}._model.0`
+        -> [LayerNorm(eps 1e-3) `{prefix}._model.1`] -> act"""
+        if not cfg:
+            return None
+        block = LayerNormAct(self.group, f"{prefix}._model.1", RNN_LN_EPS, self.act) if cfg[1] else Act(self.act)
+        return Stack(self.ops, [(Linear.of(self.group, f"{prefix}._model.0.weight"), block)])
 
     # ------------------------------------------------------------------ buffers for B sequences of T steps
     def seq_buffers(self, T: int, B: int) -> dict:
@@ -128,8 +119,8 @@ class RecurrentPPOEngine(PPOEngine):
         b["feat"] = b["xin"][:, :, :self.feat_dim]      # the encoders write their columns in place
         for name, mlp in (("pre", self.pre_mlp), ("post", self.post_mlp)):
             if mlp is not None:
-                b[name + "_y"], b["d" + name + "_y"] = f(1, N, mlp.dense), f(1, N, mlp.dense)
-                b[name + "_pre"] = f(1, N, mlp.dense) if mlp.ln is not None else None
+                dense = mlp.layers[0][0].W.shape[1]
+                b[name + "_y"], b["d" + name + "_y"], b[name] = f(1, N, dense), f(1, N, dense), mlp.acts(N)
         b["xw"], b["hbuf"], b["c0"] = f(T, B, G), f(T + 1, B, H), f(B, H)
         b["gates"], b["cs"], b["dout"], b["dgates"] = f(T, B, G), f(T, B, H), f(T, B, H), f(T, B, G)
         b["lengths"] = torch.ones(B, dtype=torch.int32, device=self.device)
@@ -138,15 +129,6 @@ class RecurrentPPOEngine(PPOEngine):
         return b
 
     # ------------------------------------------------------------------ forward
-    def _dense_fwd(self, m: _Dense, b: dict, name: str, x):
-        y = b[name + "_y"]
-        if m.ln is not None:
-            self.ops.bgemm(x, m.W.transpose(1, 2), b[name + "_pre"], bias=m.b)
-            self.ops.ln_act_fwd(b[name + "_pre"][0], m.ln[0], m.ln[1], RNN_LN_EPS, ACT_CODE[m.act], y[0])
-        else:
-            self.ops.bgemm(x, m.W.transpose(1, 2), y, bias=m.b, epi=m.act)
-        return y
-
     def seq_forward(self, b: dict, rgb, x_state, prev_actions, rgb_normalized: bool = False, keep: bool = True,
                     hT=None, cT=None, actor: bool = True, critic: bool = True):
         """RecurrentPPOAgent.forward up to the head / value outputs for the sequences of buffer set `b`, whose
@@ -158,19 +140,21 @@ class RecurrentPPOEngine(PPOEngine):
         o.copy(prev_actions.reshape(N, -1), b["xin"][0][:, self.feat_dim:])
         x = b["xin"]
         if self.pre_mlp is not None:
-            x = self._dense_fwd(self.pre_mlp, b, "pre", x)
+            self.pre_mlp.forward(x, b["pre"], b["pre_y"])
+            x = b["pre_y"]
         o.copy(self.b_ih, self.bsum)
         o.axpy(self.b_hh, self.bsum)
-        o.bgemm(x, self.W_ih.transpose(1, 2), b["xw"].view(1, N, -1), bias=self.bsum.unsqueeze(0))
+        self.W_ih.forward(o, x, b["xw"].view(1, N, -1))
         o.lstm_seq_fwd(b["xw"], self.W_hh, b["hbuf"][0], b["c0"], b["lengths"], b["hbuf"][1:],
                        b["gates"] if keep else None, b["cs"] if keep else None, hT, cT)
         y = b["hbuf"][1:].view(1, N, self.H)
         if self.post_mlp is not None:
-            y = self._dense_fwd(self.post_mlp, b, "post", y)
+            self.post_mlp.forward(y, b["post"], b["post_y"])
+            y = b["post_y"]
         if critic:
-            self._mlp_fwd(self.critic, b, y, b["values"])
+            self.critic.forward(y, b["critic"], b["values"])
         if actor:
-            self._mlp_fwd(self.actor, b, y, b["head"])
+            self.actor.forward(y, b["actor"], b["head"])
         return y
 
     # ------------------------------------------------------------------ one minibatch
@@ -221,50 +205,29 @@ class RecurrentPPOEngine(PPOEngine):
                           self.head_dims, 0, hp["clip_vloss"], hp["normalize_advantages"], hp["clip_coef"],
                           hp["vf_coef"], hp["ent_coef"])
         # ---- backward: actor, critic -> gradient w.r.t. the RNN output (post-MLP output)
-        post = self.post_mlp
-        dy = b["dpost_y"] if post is not None else b["dout"].view(1, N, self.H)
-        epi = "d" + post.act if (post is not None and post.ln is None) else "none"
-        aux = b["post_y"] if epi != "none" else None
-        for j, (st, dout) in enumerate(((self.actor, b["dhead"]), (self.critic, b["dvalues"]))):
-            dpre0, l0 = self._mlp_bwd(st, b, dout), st.lins[0]
-            o.bgemm(dpre0.transpose(1, 2), y, l0.gW, rsum=l0.gb)
-            o.bgemm(dpre0, l0.W, dy, aux=aux, epi=epi, accumulate=j > 0)
+        post, pre = self.post_mlp, self.pre_mlp
         h_out = b["hbuf"][1:].view(1, N, self.H)
+        dy = [(b["dpost_y"], None, *post.layers[0][1].dx_epi(b["post_y"])) if post is not None else
+              (b["dout"].view(1, N, self.H), None, "none", None)]
+        for j, (name, dout) in enumerate((("actor", b["dhead"]), ("critic", b["dvalues"]))):
+            getattr(self, name).backward(dout, y, b[name], dy, accumulate=j > 0)
         if post is not None:
-            self._dense_bwd(post, b, "post", h_out)
-            o.bgemm(b["dpost_y"], post.W, b["dout"].view(1, N, self.H))
+            post.backward(b["dpost_y"], h_out, b["post"], [(b["dout"].view(1, N, self.H), None, "none", None)])
         # ---- LSTM: one backward-through-time launch, then the dense products over all N rows
         o.lstm_seq_bwd(b["dout"], self.W_hh, b["gates"], b["cs"], b["c0"], b["lengths"], b["dgates"])
         dg = b["dgates"].view(1, N, 4 * self.H)
-        x = b["pre_y"] if self.pre_mlp is not None else b["xin"]
-        o.bgemm(dg.transpose(1, 2), x, self.gW_ih, rsum=self.gb_ih.unsqueeze(0))
+        self.W_ih.weight_grad(o, dg, b["pre_y"] if pre is not None else b["xin"])
         o.copy(self.gb_ih, self.gb_hh)
         o.bgemm(dg.transpose(1, 2), b["hbuf"][:-1].view(1, N, self.H), self.gW_hh)
-        if self.pre_mlp is not None:
-            pm = self.pre_mlp
-            pepi = "d" + pm.act if pm.ln is None else "none"
-            o.bgemm(dg, self.W_ih, b["dpre_y"], aux=b["pre_y"] if pm.ln is None else None, epi=pepi)
-            self._dense_bwd(pm, b, "pre", b["xin"])
-            dfirst, Wfirst = b["dpre_y"], pm.W
-        else:
-            dfirst, Wfirst = dg, self.W_ih
         # ---- feature gradient (image columns masked by the fc ReLU), encoders, clip + Adam
-        F_, feat = self.F, b["feat"]
-        if F_:
-            o.bgemm(dfirst, Wfirst[:, :, :F_], b["dfeat"][:, :, :F_], aux=feat[:, :, :F_], epi="drelu")
-        if self.Mf:
-            o.bgemm(dfirst, Wfirst[:, :, F_:self.feat_dim], b["dfeat"][:, :, F_:])
+        feats = self.feature_grads(b, self.feat_dim)
+        if pre is not None:
+            self.W_ih.input_grad(o, dg, [(b["dpre_y"], None, *pre.layers[0][1].dx_epi(b["pre_y"]))])
+            pre.backward(b["dpre_y"], b["xin"], b["pre"], feats)
+        else:
+            self.W_ih.input_grad(o, dg, feats)
         self._encoder_bwd(b, x_state)
         self._optimizer_step()
-
-    def _dense_bwd(self, m: _Dense, b: dict, name: str, x):
-        """b["d<name>_y"] holds the gradient w.r.t. the block's output (already times act' when there is no
-        LayerNorm); turn it into the Linear output gradient in place and write the weight / LayerNorm gradients."""
-        d = b["d" + name + "_y"]
-        if m.ln is not None:
-            gam, bet, dgam, dbet = m.ln
-            self.ops.ln_act_bwd(b[name + "_pre"][0], gam, bet, RNN_LN_EPS, ACT_CODE[m.act], d[0], d[0], dgam, dbet)
-        self.ops.bgemm(d.transpose(1, 2), x, m.gW, rsum=m.gb)
 
     def train(self, data: Dict[str, torch.Tensor], index_batches: Sequence[Sequence[int]], on_minibatch=None,
               prepared: Optional[dict] = None):

@@ -98,14 +98,10 @@ class SACPlayer:
         E = x.shape[0]
         if E not in self._bufs:
             f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=e.device)  # noqa: E731
-            self._bufs[E] = (f(1, E, e.Ha), f(1, E, e.Ha), f(1, E, 2 * e.A), f(E, e.A), f(E), f(E, e.A),
+            self._bufs[E] = (e.pi.acts(E, grads=False), f(1, E, 2 * e.A), f(E, e.A), f(E), f(E, e.A),
                              torch.zeros(1, dtype=torch.int32, device=e.device))
-        a1, a2, head, eps, logp, act, ctr = self._bufs[E]
-        w = e._actor_views(e.actor.views)
-        t = lambda W: W.transpose(1, 2)  # noqa: E731
-        o.bgemm(x.unsqueeze(0), t(w["W0"]), a1, bias=w["b0"], epi="relu")
-        o.bgemm(a1, t(w["W1"]), a2, bias=w["b1"], epi="relu")
-        o.bgemm(a2, t(w["W2"]), head, bias=w["b2"])
+        acts, head, eps, logp, act, ctr = self._bufs[E]
+        e.pi.forward(x.unsqueeze(0), acts, head)
         if greedy:
             eps.zero_()                                       # x_t = mean  ->  tanh(mean) * scale + bias
         else:

@@ -19,6 +19,7 @@ from typing import Dict, Optional
 
 import torch
 
+from sheeprl_b200.dense import Act, Linear, Stack, stacked
 from sheeprl_b200.params import FlatGroup
 
 
@@ -41,6 +42,8 @@ def sac_param_shapes(obs_dim: int, act_dim: int, hidden_actor: int, hidden_criti
 
 
 class SACEngine:
+    ACTOR_LOSS = "sac_actor_loss"                     # the policy loss on the min over the critics
+
     def __init__(self, obs_dim: int, act_dim: int, hidden_actor: int, hidden_critic: int, n_critics: int, batch: int,
                  gamma: float, tau: float, alpha: float, action_low, action_high, opt_actor: dict, opt_qf: dict,
                  opt_alpha: dict, device, ops, seed: int = 0):
@@ -66,61 +69,57 @@ class SACEngine:
         # (tail minibatch of a chunk) and must not rewind the stream
         self.noise_counter = torch.zeros(1, dtype=torch.int32, device=self.device)
         self.metrics = torch.zeros(3, dtype=torch.float32, device=self.device)      # value, policy, alpha loss
+        lin = lambda k: Linear.of(self.actor, k)  # noqa: E731
+        self.pi = Stack(ops, [(lin("model._model.0.weight"), Act("relu")), (lin("model._model.2.weight"), Act("relu")),
+                              (lin("head.weight"), Act("none"))])
+        self.q_online = self._critic_stack(self.qf.flat, self.qf.grad)
+        self.q_target = self._critic_stack(self.qf_target.flat)
         self._alloc()
 
     def _param_shapes(self):
         return sac_param_shapes(self.O, self.A, self.Ha, self.Hc, self.n)
 
+    def _critic_stack(self, flat: torch.Tensor, grad: Optional[torch.Tensor] = None) -> Stack:
+        """the n critics bound to `flat` (and `grad`) as one stack: [n, ...] views with the constant inter-critic stride"""
+        n, off, shapes = self.n, self.qf.offsets, self.qf.shapes
+        lin = self._critic_linears()
+        stride = off[f"1.model._model.{lin[0]}.weight"] - off[f"0.model._model.{lin[0]}.weight"] if n > 1 else flat.numel()
+
+        def v(f, key):
+            key = f"0.model._model.{key}"
+            return None if f is None else stacked(f, off[key], n, stride, shapes[key])
+
+        def linear(i):
+            return Linear(v(flat, f"{i}.weight"), v(flat, f"{i}.bias"), v(grad, f"{i}.weight"), v(grad, f"{i}.bias"))
+
+        blocks = [self._critic_block(j, lambda key: (v(flat, key), v(grad, key))) for j in range(2)] + [Act("none")]
+        return Stack(self.ops, [(linear(i), blk) for i, blk in zip(lin, blocks)])
+
+    def _critic_linears(self):
+        """indices of the critic MLP's Linears in `model._model`"""
+        return 0, 2, 4
+
+    def _critic_block(self, j: int, views):
+        """what follows the critics' hidden Linear j; views(key) -> (parameter, gradient) [n, ...] views"""
+        return Act("relu")
+
     # ------------------------------------------------------------------ buffers
     def _alloc(self):
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.device)  # noqa: E731
-        B, O, A, n, Ha, Hc = self.B, self.O, self.A, self.n, self.Ha, self.Hc
+        B, O, A, n = self.B, self.O, self.A, self.n
         self.x_next, self.x_cur, self.x_pi = f(B, O + A), f(B, O + A), f(B, O + A)
-        self.a1, self.a2, self.head = f(1, B, Ha), f(1, B, Ha), f(1, B, 2 * A)
-        self.c1, self.c2, self.q = f(n, B, Hc), f(n, B, Hc), f(n, B, 1)
+        self.pi_acts, self.head, self.q_acts, self.q = self.pi.acts(B), f(1, B, 2 * A), self.q_online.acts(B), f(n, B, 1)
         self.logp, self.tanh_y, self.y = f(B), f(B, A), f(B)
-        self.dq, self.dc2, self.dc1, self.dact = f(n, B, 1), f(n, B, Hc), f(n, B, Hc), f(n, B, A)
-        self.dhead, self.da2, self.da1 = f(1, B, 2 * A), f(1, B, Ha), f(1, B, Ha)
+        self.dq, self.dact, self.dhead = f(n, B, 1), f(n, B, A), f(1, B, 2 * A)
         self.eps_next, self.eps_cur = f(B, A), f(B, A)
         self.norm_out = f(1)
         self.zero_normsq = torch.zeros(1, dtype=torch.float64, device=self.device)
-        # batched views of the critics' parameters: [n, out, in] with the constant inter-critic stride
-        self._qv = self._critic_views(self.qf.flat)
-        self._qg = self._critic_views(self.qf.grad)
-        self._tv = self._critic_views(self.qf_target.flat)
-
-    def _critic_views(self, flat: torch.Tensor):
-        n, Hc, I = self.n, self.Hc, self.O + self.A
-        off = self.qf.offsets
-        stride = off["1.model._model.0.weight"] - off["0.model._model.0.weight"] if n > 1 else flat.numel()
-
-        def v(key, rows, cols):
-            return torch.as_strided(flat, (n, rows, cols), (stride, cols, 1), off[f"0.model._model.{key}"])
-
-        return {"W0": v("0.weight", Hc, I), "b0": v("0.bias", 1, Hc)[:, 0], "W1": v("2.weight", Hc, Hc),
-                "b1": v("2.bias", 1, Hc)[:, 0], "W2": v("4.weight", 1, Hc), "b2": v("4.bias", 1, 1)[:, 0]}
-
-    def _actor_views(self, views):
-        u = lambda k: views[k].unsqueeze(0)  # noqa: E731
-        return {"W0": u("model._model.0.weight"), "b0": u("model._model.0.bias"), "W1": u("model._model.2.weight"),
-                "b1": u("model._model.2.bias"), "W2": u("head.weight"), "b2": u("head.bias")}
 
     # ------------------------------------------------------------------ networks
     def _actor_fwd(self, obs: torch.Tensor, eps: torch.Tensor, action_out: torch.Tensor, save_tanh: bool):
-        o, w = self.ops, self._actor_views(self.actor.views)
-        t = lambda W: W.transpose(1, 2)  # noqa: E731
-        o.bgemm(obs.unsqueeze(0), t(w["W0"]), self.a1, bias=w["b0"], epi="relu")
-        o.bgemm(self.a1, t(w["W1"]), self.a2, bias=w["b1"], epi="relu")
-        o.bgemm(self.a2, t(w["W2"]), self.head, bias=w["b2"])
-        o.sac_sample_fwd(self.head[0], eps, self.scale, self.abias, action_out, self.logp,
-                         self.tanh_y if save_tanh else None)
-
-    def _critic_fwd(self, w, x: torch.Tensor):
-        o = self.ops
-        t = lambda W: W.transpose(1, 2)  # noqa: E731
-        o.bgemm(x.unsqueeze(0), t(w["W0"]), self.c1, bias=w["b0"], epi="relu")
-        o.bgemm(self.c1, t(w["W1"]), self.c2, bias=w["b1"], epi="relu")
-        o.bgemm(self.c2, t(w["W2"]), self.q, bias=w["b2"])
+        self.pi.forward(obs.unsqueeze(0), self.pi_acts, self.head)
+        self.ops.sac_sample_fwd(self.head[0], eps, self.scale, self.abias, action_out, self.logp,
+                                self.tanh_y if save_tanh else None)
 
     def _adam(self, group: FlatGroup, opt: dict, name: str):
         if self.allreduce is not None:
@@ -154,12 +153,12 @@ class SACEngine:
         la = self.alpha.views["log_alpha"]
         # ---- soft-critic update (sac.py:45-53)
         self._actor_fwd(nobs, eps_next, self.x_next[:, O:], save_tanh=False)
-        self._critic_fwd(self._tv, self.x_next)
+        self.q_target.forward(self.x_next.unsqueeze(0), self.q_acts, self.q)
         o.sac_target(self.q[:, :, 0], self.logp, data["rewards"].reshape(-1), data["terminated"].reshape(-1), la,
                      self.gamma, self.y)
-        self._critic_fwd(self._qv, self.x_cur)
+        self.q_online.forward(self.x_cur.unsqueeze(0), self.q_acts, self.q)
         o.sac_critic_loss(self.q[:, :, 0], self.y, self.dq[:, :, 0], self.metrics[0:1])
-        self._critic_bwd_weights(self._qv, self._qg, self.x_cur)
+        self.q_online.backward(self.dq, self.x_cur.unsqueeze(0), self.q_acts)
         self._adam(self.qf, self.opt["qf"], "qf")
         # ---- target EMA (sac.py:55-57)
         if do_ema:
@@ -167,44 +166,23 @@ class SACEngine:
         # ---- actor update (sac.py:59-66) and temperature (sac.py:68-73)
         self._actor_update(obs, eps_cur)
 
-    def _actor_update(self, obs: torch.Tensor, eps_cur: torch.Tensor):
-        """one actor and one temperature step on `obs` (whose copy already sits in x_pi's observation columns)"""
-        o, O = self.ops, self.O
+    def _actor_update(self, obs: torch.Tensor, eps_cur: torch.Tensor, masks: Optional[torch.Tensor] = None):
+        """one actor and one temperature step on `obs` (whose copy already sits in x_pi's observation columns): the
+        policy and temperature losses on the critics' q of x_pi, then the critics' input gradient w.r.t. the action
+        columns only (dact; no critic parameter gradients) and the actor's backward.  masks: the critics' dropout masks"""
+        o, x_pi = self.ops, self.x_pi.unsqueeze(0)
         la = self.alpha.views["log_alpha"]
-        t = lambda W: W.transpose(1, 2)  # noqa: E731
-        self._actor_fwd(obs, eps_cur, self.x_pi[:, O:], save_tanh=True)
-        self._policy_loss_grad()
+        self._actor_fwd(obs, eps_cur, self.x_pi[:, self.O:], save_tanh=True)
+        self.q_online.forward(x_pi, self.q_acts, self.q, masks)
+        getattr(o, self.ACTOR_LOSS)(self.q[:, :, 0], self.logp, la, self.target_entropy, self.dq[:, :, 0],
+                                    self.metrics[1:2], self.metrics[2:3], self.alpha.grad[0:1])
+        self.q_online.backward(self.dq, x_pi, self.q_acts, [(self.dact, slice(self.O, None), "none", None)], wgrad=False,
+                               masks=masks)
         o.sac_sample_bwd(self.head[0], eps_cur, self.tanh_y, self.scale, self.dact, la, self.dhead[0])
-        aw, ag = self._actor_views(self.actor.views), self._actor_views(self.actor.gviews)
-        o.bgemm(t(self.dhead), self.a2, ag["W2"], rsum=ag["b2"])
-        o.bgemm(self.dhead, aw["W2"], self.da2, aux=self.a2, epi="drelu")
-        o.bgemm(t(self.da2), self.a1, ag["W1"], rsum=ag["b1"])
-        o.bgemm(self.da2, aw["W1"], self.da1, aux=self.a1, epi="drelu")
-        o.bgemm(t(self.da1), obs.unsqueeze(0), ag["W0"], rsum=ag["b0"])
+        self.pi.backward(self.dhead, obs.unsqueeze(0), self.pi_acts)
         self._adam(self.actor, self.opt["actor"], "actor")
         # temperature: gradient written by the policy loss kernel
         self._adam(self.alpha, self.opt["alpha"], "alpha")
-
-    def _policy_loss_grad(self):
-        """policy + temperature losses on the critics' q of x_pi (min over the critics), dq, the log_alpha gradient and
-        the input gradient of the critics w.r.t. the action columns only (dact)"""
-        o, O, w = self.ops, self.O, self._qv
-        la = self.alpha.views["log_alpha"]
-        self._critic_fwd(w, self.x_pi)
-        o.sac_actor_loss(self.q[:, :, 0], self.logp, la, self.target_entropy, self.dq[:, :, 0], self.metrics[1:2],
-                         self.metrics[2:3], self.alpha.grad[0:1])
-        o.bgemm(self.dq, w["W2"], self.dc2, aux=self.c2, epi="drelu")
-        o.bgemm(self.dc2, w["W1"], self.dc1, aux=self.c1, epi="drelu")
-        o.bgemm(self.dc1, w["W0"][:, :, O:], self.dact)
-
-    def _critic_bwd_weights(self, w, g, x):
-        o = self.ops
-        t = lambda W: W.transpose(1, 2)  # noqa: E731
-        o.bgemm(t(self.dq), self.c2, g["W2"], rsum=g["b2"])
-        o.bgemm(self.dq, w["W2"], self.dc2, aux=self.c2, epi="drelu")
-        o.bgemm(t(self.dc2), self.c1, g["W1"], rsum=g["b1"])
-        o.bgemm(self.dc2, w["W1"], self.dc1, aux=self.c1, epi="drelu")
-        o.bgemm(t(self.dc1), x.unsqueeze(0), g["W0"], rsum=g["b0"])
 
     # ------------------------------------------------------------------ state
     def metrics_dict(self) -> Dict[str, torch.Tensor]:
