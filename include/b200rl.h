@@ -226,6 +226,36 @@ int b200rl_rssm_scan_check(const b200rl_rssm_scan_args* args, int backward);
 int b200rl_rssm_scan_error(const void* workspace, cudaStream_t stream);
 /* cycle counters (2 x 32 int64: CTA 0, CTA 1) accumulated per phase by the last launch on `workspace` */
 int b200rl_rssm_scan_profile(const void* workspace, long long* out64, cudaStream_t stream);
+/* Persistent GRU-only scan for the decoupled RSSM (DecoupledRSSM agent.py:501-593, dreamer_v3.py:115-129): the
+ * posterior does not depend on h there, so x = SiLU(LN(W_in [z, a])) and its share x W_g[:, R:]^T of the gate
+ * pre-activation are batched over all T*B rows by the caller; the kernels run what is left on the recurrence,
+ * h_in = (1-f) h_{t-1} + f h0, g_pre += h_in W_g[:, :R]^T, LayerNorm over 3R, gate, for all T steps in one cooperative
+ * launch (rssm_scan.cu; same construction and helpers as b200rl_rssm_scan_*).  Requires B <= 16, R even and <= 1024,
+ * and the per-CTA W_g[:, :R] slice to fit in 227 KB of shared memory.  b200rl_gru_scan_check answers that per direction,
+ * reads no pointer and launches nothing; the launches refuse the same shapes (and a short workspace) before launching.
+ * b200rl_rssm_scan_error reads the error word of this workspace too. */
+typedef struct b200rl_gru_scan_args {
+  int T, B, R, ld_wg, ld_lat, lat_off;        /* h_t is written to latent[t*B + b, lat_off : lat_off + R] */
+  float eps;
+  const float *W_g, *lng_g, *lng_b;           /* [3R, ld_wg], columns [:R] are read; GRU LayerNorm weight, bias [3R] */
+  const float *h0, *first;                    /* [R] tanh(initial_recurrent_state); [T*B] */
+  float* g_pre;                               /* [T*B, 3R] in: x's share of the pre-activation; out: all of it */
+  float *g_ln, *h_in, *latent;                /* [T*B, 3R]; [T*B, R]; [T*B, ld_lat] */
+  void* workspace;
+  long long workspace_bytes;
+} b200rl_gru_scan_args;
+/* d_latent [T*B, ld_lat] (its h columns are read); q_g = g_pre W_g[:, :R] [T*B, R] over all rows (lets the consumer of
+ * the LayerNorm gradient apply the LayerNorm-backward correction by linearity); outputs d_g_ln [T*B, 3R], the gradient
+ * of the LayerNorm's output (the batched LayerNorm-backward kernel turns it into d_g_pre afterwards), and d_h0 [R]. */
+typedef struct b200rl_gru_scan_grads {
+  const float *d_latent, *q_g;
+  float *d_g_ln, *d_h0;
+} b200rl_gru_scan_grads;
+long long b200rl_gru_scan_workspace_bytes(int T, int B, int R);
+int b200rl_gru_scan_fwd(const b200rl_gru_scan_args* args, cudaStream_t stream);
+/* must follow b200rl_gru_scan_fwd on the same workspace (uses its saved LayerNorm statistics) */
+int b200rl_gru_scan_bwd(const b200rl_gru_scan_args* args, const b200rl_gru_scan_grads* grads, cudaStream_t stream);
+int b200rl_gru_scan_check(const b200rl_gru_scan_args* args, int backward);
 
 /* ---- losses (value + seed gradient) -----------------------------------------------------------------
  * distribution.py:212-276 (MSE, two-hot on symlog), Bernoulli continue head loss.py:77, lambda returns

@@ -111,9 +111,10 @@ class PlayerDV3:
         e._recurrent_forward(self.stochastic_state[0], self.actions[0], self.recurrent_state[0], e.x_pre, e.x_act,
                              e.g_pre, e.g_ln, self._h_next)
         self.recurrent_state[0].copy_(self._h_next)
-        # posterior from [h, embed] (agent.py:451-465) and its sample
+        # posterior from [h, embed] (agent.py:451-465; decoupled RSSM: from the embedding alone, :682-683) and its sample
         e._project_embedding(e.rp_pre)
-        e._posterior_forward(self._h_next, e.rp_pre, e.rp_act, e.post_raw, nz, self.stochastic_state[0])
+        e._posterior_forward(None if e.decoupled else self._h_next, e.rp_pre, e.rp_act, e.post_raw, nz,
+                             self.stochastic_state[0])
         # actor on [z, h] (agent.py:783-837)
         lat = e.latent                                                       # [E, Z+R] scratch row block
         ops.copy(self.stochastic_state[0], lat[:, :Z])

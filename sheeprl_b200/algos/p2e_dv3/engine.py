@@ -51,6 +51,10 @@ class P2EDV3Engine(DV3Engine):
 
     def __init__(self, cfg, actions_dim: Sequence[int], in_channels: int = 3, device="cuda", ops=None,
                  is_continuous: bool = False, mlp_dims=None):
+        if cfg.algo.world_model.decoupled_rssm:
+            raise NotImplementedError(
+                "Plan2Explore cannot run with decoupled_rssm: the reference's exploration train() calls the five-argument "
+                "RSSM.dynamic (p2e_dv3_exploration.py:136), which DecoupledRSSM does not have")
         super().__init__(cfg, actions_dim, in_channels, device, ops, is_continuous=is_continuous, mlp_dims=mlp_dims)
         a = cfg.algo
         N, H, L, A, Z = self.N, self.H, self.L, self.A, self.Z

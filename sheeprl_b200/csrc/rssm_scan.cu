@@ -1358,6 +1358,378 @@ int workspace_check(const b200rl_rssm_scan_args& a) {
   return B200RL_OK;
 }
 
+// =====================================================================================================
+// GRU-only scan (decoupled RSSM, agent.py:501-593 / dreamer_v3.py:115-129).  The posterior is a function of the embedding
+// alone there, so z of every step, x = SiLU(LN(W_in [z, a])) and x's share of the gate pre-activation are batched products
+// over all T*B rows outside these kernels; what stays on the recurrence is
+//   forward   h_in = (1-f) h_{t-1} + f h0 --W_g[:, :R]--> (+ x share) g_pre --LN over 3R--> gates --> h_t
+//   backward  dh_t --gates--> d_g_ln --LN--> d_g_pre --W_g[:, :R]--> dh_in --(1-f) / f--> dh_{t-1}, d_h0
+// Same construction as the kernels above and on their helpers.  A CTA owns the r, c, u columns of the SAME h columns, so
+// the gate is local and its W_g[:, :R] slice stays in shared memory for all T steps.  Two hand-offs per forward step (the
+// LayerNorm partial statistics; the h rows — the statistics do not ride with the values: every CTA would then have to
+// read all 3R pre-activations of every row instead of 128 partials) and one per backward step (the LayerNorm-backward
+// inputs dxh of all 3R columns together with their row sums; the correction is applied by the consumer through
+// q_g = g_pre W_g[:, :R], one batched product in front of the kernel).
+// =====================================================================================================
+struct GruLL { size_t s, h, c, sc, total; };      // offsets (u64 elements), double-buffered by step parity
+__host__ __device__ inline GruLL make_gru_ll(int R) {
+  GruLL g;
+  size_t o = 0;
+  g.s = o;  o += 2 * (size_t)MAXB * SCAN_G * 2;   // forward: partial statistics of the GRU LayerNorm
+  g.h = o;  o += 2 * (size_t)MAXB * R;            //          h rows
+  g.c = o;  o += 2 * (size_t)MAXB * 3 * R;        // backward: dxh of the GRU LayerNorm
+  g.sc = o; o += 2 * (size_t)MAXB * SCAN_G * 2;   //           per-CTA row sums (sum dxh, sum dxh*xh)
+  g.total = o;
+  return g;
+}
+// workspace: [header 256 B (error word at +64, as above) | LL region (zeroed at every launch) | (mean, rstd) of every row]
+__host__ __device__ inline size_t gru_ws_bytes(int T, int B, int R) {
+  return WS_HEADER + make_gru_ll(R).total * sizeof(u64) + sizeof(float) * 2 * (size_t)T * B + 256;
+}
+
+struct GeoG {
+  int ngh, sR, ldp;
+  int pw;                        // backward: LayerNorm parts (of 3) staged per product pass — all three where they fit
+  int oW, oX, oPart, oAcc, oSt, oDhc, oPar, oLn, oMisc, oTab, total;
+};
+__host__ __device__ inline GeoG make_geo_g(int R, int cta, bool backward) {
+  GeoG g;
+  g.ngh = owned_groups(R, cta);
+  g.sR = r4(R);
+  const int mh = owned_groups(R, 0);
+  g.ldp = backward ? mh * 4 : mh * 12;
+  for (g.pw = backward ? 3 : 1;; g.pw = 1) {
+    int o = 0;
+    g.oW = o;    o += mh * 12 * g.sR;            // fwd [ngh*12][sR] rows of W_g[:, :R]; bwd [ngh*4][3*sR] its columns
+    g.oX = o;    o += MAXB * g.pw * g.sR;        // fwd h rows; bwd dxh rows
+    g.oPart = o; o += KS_MAX * MAXB * g.ldp;
+    g.oAcc = o;  o += MAXB * g.ldp;
+    g.oSt = o;   o += backward ? 2 * MAXB * mh * 12 : 0;
+    g.oDhc = o;  o += backward ? MAXB * mh * 4 : 0;
+    g.oPar = o;  o += backward ? mh * 4 : g.sR;  // fwd h0; bwd column sums of the weight slice
+    g.oLn = o;   o += mh * 24;                   // LayerNorm weight, bias of the owned columns: [part][gamma, beta][col]
+    g.oMisc = o; o += 96;
+    g.oTab = o;  o += SCAN_G;
+    g.total = o;
+    if (g.pw == 1 || sizeof(float) * (size_t)o <= 227 * 1024) break;
+  }
+  return g;
+}
+
+// Merges the per-CTA (mean, M2) partials of one row's LayerNorm statistics (Chan); the whole warp works on the row.
+// `cnt[c]`: values CTA c contributed, `n` their total.
+__device__ __noinline__ void merge_row_stats(const u64* base, unsigned tag, const int* cnt, float n, float eps, int lane,
+                                                Spin& sp, float& mean, float& rstd) {
+  u64 x[SCAN_G / 32], y[SCAN_G / 32];
+#pragma unroll
+  for (int i = 0; i < SCAN_G / 32; ++i) ll_load2(base + (lane + 32 * i) * 2, x[i], y[i]);
+  for (;;) {                                     // stale partials are re-polled together
+    bool stale = false;
+#pragma unroll
+    for (int i = 0; i < SCAN_G / 32; ++i)
+      if ((unsigned)(x[i] >> 32) != tag || (unsigned)(y[i] >> 32) != tag) stale = true;
+    if (!stale || sp.fail()) break;
+#pragma unroll
+    for (int i = 0; i < SCAN_G / 32; ++i)
+      if ((unsigned)(x[i] >> 32) != tag || (unsigned)(y[i] >> 32) != tag) ll_load2(base + (lane + 32 * i) * 2, x[i], y[i]);
+  }
+  float sm_ = 0.f;
+#pragma unroll
+  for (int i = 0; i < SCAN_G / 32; ++i) sm_ += (float)cnt[lane + 32 * i] * __uint_as_float((unsigned)x[i]);
+  mean = warp_sum(sm_) / n;
+  float m2 = 0.f;
+#pragma unroll
+  for (int i = 0; i < SCAN_G / 32; ++i) {
+    const float d = __uint_as_float((unsigned)x[i]) - mean;
+    m2 += __uint_as_float((unsigned)y[i]) + (float)cnt[lane + 32 * i] * d * d;
+  }
+  rstd = rsqrtf(warp_sum(m2) / n + eps);
+}
+
+__global__ void __launch_bounds__(SCAN_NT, 1) gru_scan_fwd_kernel(const b200rl_gru_scan_args a) {
+  extern __shared__ __align__(16) float sm[];
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int cta = blockIdx.x;
+  const int T = a.T, B = a.B, R = a.R;
+  const GeoG g = make_geo_g(R, cta, false);
+  const GruLL L = make_gru_ll(R);
+  int* error = (int*)((char*)a.workspace + 64);
+  u64* ll = (u64*)((char*)a.workspace + WS_HEADER);
+  float* ln_stats = (float*)(ll + L.total);
+  float* Wg = sm + g.oW;        // [ngh*12][sR]  rows: (group, part r/c/u, col-in-group)
+  float* Xh = sm + g.oX;        // [MAXB][sR]  h rows (carried from one step to the next)
+  float* PART = sm + g.oPart;
+  float* ACC = sm + g.oAcc;     // [MAXB][ldp] finished g_pre columns (for the row statistics)
+  float* H0 = sm + g.oPar;      // [R] tanh(initial_recurrent_state)
+  float* LNP = sm + g.oLn;      // [3][2][nh4] (read from shared memory at the gate: values kept in registers across the
+                                // product / receive calls were spilled)
+  float* misc = sm + g.oMisc;   // [0,16) first flags; [16,32) mean; [32,48) rstd
+  int* nctab = (int*)(sm + g.oTab);   // LayerNorm values per CTA
+  const int ldp = g.ldp;
+  Spin sp;
+  sp.init(error);
+
+  // ---------------- prologue: the weight slice and h0 -> shared memory (read from HBM once per scan)
+  for (int e = tid; e < g.total; e += SCAN_NT) sm[e] = 0.f;
+  __syncthreads();
+  for (int gi = 0; gi < g.ngh; ++gi)
+    for (int part = 0; part < 3; ++part)
+      load_rows4(Wg + (size_t)(gi * 3 + part) * 4 * g.sR, g.sR, 0, a.W_g + (size_t)part * R * a.ld_wg, a.ld_wg,
+                 (cta + gi * SCAN_G) * 4, R, 0, R, g.sR, tid);
+  for (int k = tid; k < R; k += SCAN_NT) H0[k] = a.h0[k];
+  for (int c = tid; c < SCAN_G; c += SCAN_NT) nctab[c] = 3 * owned_cols(R, c);
+  // fixed element assignments (no index arithmetic inside the time loop)
+  const int nh4 = g.ngh * 4, nh12 = g.ngh * 12;
+  const Slot sH = make_slot(tid, nh4, B, cta, R);           // gate / h element
+  const int pb = nh12 > 0 ? tid / nh12 : 0, pc = tid - pb * nh12;   // g_pre element: (group, part, j) of the 12*ngh products
+  const int pcol = (cta + (pc / 12) * SCAN_G) * 4 + (pc & 3), ppart = (pc % 12) >> 2;
+  const bool pok = nh12 > 0 && pb < B && pcol < R;
+  for (int e = tid; e < 3 * nh4; e += SCAN_NT) {
+    const int part = e / nh4, cj = e - part * nh4, col = (cta + (cj >> 2) * SCAN_G) * 4 + (cj & 3);
+    LNP[(part * 2) * nh4 + cj] = col < R ? a.lng_g[part * R + col] : 0.f;
+    LNP[(part * 2 + 1) * nh4 + cj] = col < R ? a.lng_b[part * R + col] : 0.f;
+  }
+  const int ncol3 = 3 * owned_cols(R, cta);
+  float first_next = (tid < B) ? a.first[tid] : 0.f;        // is_first flags of the step about to run (threads < MAXB)
+  __syncthreads();
+
+  for (int t = 0; t < T; ++t) {
+    const size_t row0 = (size_t)t * B;
+    const int par = t & 1;
+    const unsigned tag = (unsigned)t + 1u;
+    // operands that do not depend on the chain, before the wait: flags, x's share of the pre-activation
+    if (tid < MAXB) misc[tid] = first_next;
+    if (tid < MAXB) first_next = (tid < B && t + 1 < T) ? a.first[row0 + B + tid] : 0.f;
+    const float gx = pok ? a.g_pre[(row0 + pb) * 3 * R + (size_t)ppart * R + pcol] : 0.f;
+    if (t > 0) ll_recv<8>(Xh, g.sR, ll + L.h + (size_t)(par ^ 1) * MAXB * R, R, B, R, (unsigned)t, tid, sp);
+    __syncthreads();
+    const float* fl = misc;
+    // h_in = (1-f) h_{t-1} + f h0 (agent.py:574), rows with f != 0 only
+    for (int b = 0; b < B; ++b) {
+      const float f = fl[b];
+      if (f != 0.f || t == 0)
+        for (int k = tid; k < R; k += SCAN_NT) Xh[b * g.sR + k] = (1.f - f) * ((t > 0) ? Xh[b * g.sR + k] : 0.f) + f * H0[k];
+    }
+    __syncthreads();
+    const int ksh = product(Xh, g.sR, Wg, g.sR, g.ngh * 3, R, B, PART, ldp, 0, tid);
+    __syncthreads();
+    float gpre = 0.f;
+    if (pok) {
+      gpre = gx + part_sum(PART, ldp, ksh, pb, pc);
+      ACC[pb * ldp + pc] = gpre;
+    }
+    const float hin = sH.ok ? Xh[sH.b * g.sR + sH.col] : 0.f;
+    __syncthreads();
+    for (int b = wid; b < B; b += SCAN_NW) {   // per-row partial statistics (mean, M2) over the owned valid columns
+      float s = 0.f;
+      for (int c = lane; c < nh12; c += 32)
+        if ((cta + (c / 12) * SCAN_G) * 4 + (c & 3) < R) s += ACC[b * ldp + c];
+      s = warp_sum(s);
+      const float mean = ncol3 > 0 ? s / (float)ncol3 : 0.f;
+      float m2 = 0.f;
+      for (int c = lane; c < nh12; c += 32)
+        if ((cta + (c / 12) * SCAN_G) * 4 + (c & 3) < R) { const float d = ACC[b * ldp + c] - mean; m2 = fmaf(d, d, m2); }
+      m2 = warp_sum(m2);
+      if (lane == 0) ll_store2(ll + L.s + (((size_t)par * MAXB + b) * SCAN_G + cta) * 2, mean, m2, tag);
+    }
+    if (pok) a.g_pre[(row0 + pb) * 3 * R + (size_t)ppart * R + pcol] = gpre;      // save after the hand-off
+    for (int b = wid; b < B; b += SCAN_NW) {
+      float mean, rstd;
+      merge_row_stats(ll + L.s + ((size_t)par * MAXB + b) * SCAN_G * 2, tag, nctab, (float)(3 * R), a.eps, lane, sp, mean, rstd);
+      if (lane == 0) {
+        misc[16 + b] = mean;
+        misc[32 + b] = rstd;
+        if (cta == (t % SCAN_G)) { ln_stats[(row0 + b) * 2] = mean; ln_stats[(row0 + b) * 2 + 1] = rstd; }
+      }
+    }
+    __syncthreads();
+    if (sH.ok) {                               // LayerNorm, GRU gate (models.py:396-403) -> h_t for the owned columns
+      const int b = sH.b, gi = sH.cj >> 2, j = sH.cj & 3;
+      const float mu = misc[16 + b], rstd = misc[32 + b];
+      float gl[3];
+#pragma unroll
+      for (int part = 0; part < 3; ++part)
+        gl[part] = (ACC[b * ldp + gi * 12 + part * 4 + j] - mu) * rstd * LNP[(part * 2) * nh4 + sH.cj] + LNP[(part * 2 + 1) * nh4 + sH.cj];
+      const float r = sigmoidf_(gl[0]);
+      const float c = tanhf(r * gl[1]);
+      const float u = sigmoidf_(gl[2] - 1.f);
+      const float h = u * c + (1.f - u) * hin;
+      ll_store(ll + L.h + ((size_t)par * MAXB + b) * R + sH.col, h, tag);         // hand-off first, saves after
+      a.latent[(row0 + b) * a.ld_lat + a.lat_off + sH.col] = h;
+#pragma unroll
+      for (int part = 0; part < 3; ++part) a.g_ln[(row0 + b) * 3 * R + (size_t)part * R + sH.col] = gl[part];
+      a.h_in[(row0 + b) * R + sH.col] = hin;
+    }
+    __syncthreads();
+    if (sp.dead) break;    // a hand-off timed out somewhere: bail out, never hang
+  }
+}
+
+__global__ void __launch_bounds__(SCAN_NT, 1)
+gru_scan_bwd_kernel(const b200rl_gru_scan_args a, const b200rl_gru_scan_grads q) {
+  extern __shared__ __align__(16) float sm[];
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int cta = blockIdx.x;
+  const int T = a.T, B = a.B, R = a.R;
+  const GeoG g = make_geo_g(R, cta, true);
+  const GruLL L = make_gru_ll(R);
+  int* error = (int*)((char*)a.workspace + 64);
+  u64* ll = (u64*)((char*)a.workspace + WS_HEADER);
+  const float* ln_stats = (const float*)(ll + L.total);
+  float* WgT = sm + g.oW;       // [ngh*4][3*sR] columns of W_g[:, :R] (3 parts of sR)
+  float* X = sm + g.oX;         // [MAXB][pw*sR]
+  float* PART = sm + g.oPart;
+  float* ACC = sm + g.oAcc;     // [MAXB][ldp]
+  float* ST = sm + g.oSt;       // [(b, col)][2] staged (dxh, dxh*xh)
+  float* DHC = sm + g.oDhc;     // [MAXB][nh4] dh carried to step t-1
+  float* WSG = sm + g.oPar;     // [nh4] column sums of the weight slice
+  float* LNP = sm + g.oLn;      // [3][nh4] LayerNorm weight of the owned columns
+  float* misc = sm + g.oMisc;   // [0,16) first(t); [32,48) S1; [48,64) S2; [64,96) (mu, rstd) of step t
+  float* S1 = misc + 32;
+  float* S2 = misc + 48;
+  float* LNS = misc + 64;
+  const int ldp = g.ldp, wgst = 3 * g.sR, xw = g.pw * g.sR, nh4 = g.ngh * 4;
+  Spin sp;
+  sp.init(error);
+
+  for (int e = tid; e < g.total; e += SCAN_NT) sm[e] = 0.f;
+  __syncthreads();
+  for (int gi = 0; gi < g.ngh; ++gi)
+    for (int part = 0; part < 3; ++part)
+      load_cols4(WgT + (size_t)gi * 4 * wgst, wgst, a.W_g + (size_t)part * R * a.ld_wg, a.ld_wg, (cta + gi * SCAN_G) * 4, R, R,
+                 part * g.sR, tid);
+  __syncthreads();
+  for (int j = wid; j < nh4; j += SCAN_NW) {
+    float s = 0.f;
+    for (int k = lane; k < wgst; k += 32) s += WgT[(size_t)j * wgst + k];
+    s = warp_sum(s);
+    if (lane == 0) WSG[j] = s;
+  }
+  __syncthreads();
+  const Slot sH = make_slot(tid, nh4, B, cta, R);            // dh element
+  for (int e = tid; e < 3 * nh4; e += SCAN_NT) {
+    const int part = e / nh4, cj = e - part * nh4, col = (cta + (cj >> 2) * SCAN_G) * 4 + (cj & 3);
+    LNP[part * nh4 + cj] = col < R ? a.lng_g[part * R + col] : 0.f;
+  }
+  float dh0_acc = 0.f;                                        // (threads tid < nh4) accumulated over rows in fixed order
+
+  for (int t = T - 1; t >= 0; --t) {
+    const size_t row0 = (size_t)t * B;
+    const int bt = T - 1 - t, par = bt & 1;
+    const unsigned tag = (unsigned)bt + 1u;
+    const bool last = (t == T - 1);
+    // ---------------- step-start prefetch of chain-independent inputs (registers of the element's thread)
+    if (tid < MAXB) misc[tid] = (tid < B) ? a.first[row0 + tid] : 0.f;
+    for (int e = tid; e < B * 2; e += SCAN_NT) LNS[e] = ln_stats[row0 * 2 + e];
+    float p_hin = 0.f, p_dlh = 0.f, p_qg = 0.f, p_gl[3] = {0.f, 0.f, 0.f}, p_gp[3] = {0.f, 0.f, 0.f};
+    if (sH.ok) {
+      p_hin = a.h_in[(row0 + sH.b) * R + sH.col];
+      p_dlh = q.d_latent[(row0 + sH.b) * a.ld_lat + a.lat_off + sH.col];
+      p_qg = q.q_g[(row0 + sH.b) * R + sH.col];
+#pragma unroll
+      for (int part = 0; part < 3; ++part) {
+        p_gl[part] = a.g_ln[(row0 + sH.b) * 3 * R + (size_t)part * R + sH.col];
+        p_gp[part] = a.g_pre[(row0 + sH.b) * 3 * R + (size_t)part * R + sH.col];
+      }
+    }
+    __syncthreads();
+    const float* fl = misc;
+
+    // ============ dh = d_latent_h + carry ; GRU gate backward ; dxh of the GRU LayerNorm and its row sums
+    float dhin_gate = 0.f, dgl[3] = {0.f, 0.f, 0.f};
+    if (sH.ok) {
+      const int b = sH.b;
+      const float mug = LNS[b * 2], rstdg = LNS[b * 2 + 1];
+      float dh = p_dlh;
+      if (!last) dh += DHC[b * nh4 + sH.cj];
+      const float r = sigmoidf_(p_gl[0]), cnd = tanhf(r * p_gl[1]), u = sigmoidf_(p_gl[2] - 1.f);
+      const float du = dh * (cnd - p_hin);
+      const float drc = dh * u * (1.f - cnd * cnd);
+      dgl[0] = drc * p_gl[1] * r * (1.f - r);
+      dgl[1] = drc * r;
+      dgl[2] = du * u * (1.f - u);
+      dhin_gate = dh * (1.f - u);
+#pragma unroll
+      for (int part = 0; part < 3; ++part) {
+        const float xh = (p_gp[part] - mug) * rstdg;
+        const float dxh = dgl[part] * LNP[part * nh4 + sH.cj];
+        ll_store(ll + L.c + ((size_t)par * MAXB + b) * 3 * R + (size_t)part * R + sH.col, dxh, tag);
+        ST[(b * (3 * nh4) + part * nh4 + sH.cj) * 2] = dxh;
+        ST[(b * (3 * nh4) + part * nh4 + sH.cj) * 2 + 1] = dxh * xh;
+      }
+    } else if (tid < B * nh4) {
+      const int b = tid / imax(nh4, 1), cj = tid - b * nh4;
+#pragma unroll
+      for (int part = 0; part < 3; ++part) {
+        ST[(b * (3 * nh4) + part * nh4 + cj) * 2] = 0.f;
+        ST[(b * (3 * nh4) + part * nh4 + cj) * 2 + 1] = 0.f;
+      }
+    }
+    __syncthreads();
+    send_row_sums(ST, 3 * nh4, B, ll + L.sc, par, cta, tag, tid);
+    if (sH.ok)
+#pragma unroll
+      for (int part = 0; part < 3; ++part) q.d_g_ln[(row0 + sH.b) * 3 * R + (size_t)part * R + sH.col] = dgl[part];
+
+    // ============ dh_in = d_g_pre W_g[:, :R] for the owned columns (K = 3R, in 3 / pw passes)
+    float acc_h = 0.f;
+    for (int p0 = 0; p0 < 3; p0 += g.pw) {
+      for (int part = p0; part < p0 + g.pw; ++part)
+        ll_recv<4>(X + (part - p0) * g.sR, xw, ll + L.c + (size_t)par * MAXB * 3 * R + (size_t)part * R, 3 * R, B, R, tag, tid, sp);
+      if (p0 == 0) recv_row_sums(ll + L.sc, par, 0, B, tag, 1.f / (float)(3 * R), S1, S2, tid, sp);
+      __syncthreads();
+      const int ks = product(X, xw, WgT + p0 * g.sR, wgst, g.ngh, g.pw * g.sR, B, PART, ldp, 0, tid);
+      __syncthreads();
+      if (sH.ok) acc_h += part_sum(PART, ldp, ks, sH.b, sH.cj);
+      __syncthreads();
+    }
+    float dhin_f = 0.f;
+    if (sH.ok) {
+      const int b = sH.b;
+      const float mug = LNS[b * 2], rstdg = LNS[b * 2 + 1];
+      const float wsgh = WSG[sH.cj];
+      const float p2 = rstdg * (p_qg - mug * wsgh);
+      const float dhin = dhin_gate + rstdg * (acc_h - S1[b] * wsgh - S2[b] * p2);
+      DHC[b * nh4 + sH.cj] = (1.f - fl[b]) * dhin;          // carried to step t-1 (agent.py:574 mask)
+      dhin_f = fl[b] * dhin;                                // grad of tanh(initial_recurrent_state)
+    }
+    // d_h0: sum over the rows with is_first set, fixed row order (bit-reproducible): stage through ACC
+    if (sH.ok) ACC[sH.b * ldp + sH.cj] = dhin_f;
+    __syncthreads();
+    if (tid < nh4)
+      for (int b = 0; b < B; ++b)
+        if (fl[b] != 0.f) dh0_acc += ACC[b * ldp + tid];
+    __syncthreads();
+    if (sp.dead) break;    // a hand-off timed out somewhere: bail out, never hang
+  }
+  if (tid < nh4) {
+    const int col = (cta + (tid >> 2) * SCAN_G) * 4 + (tid & 3);
+    if (col < R) q.d_h0[col] = dh0_acc;
+  }
+}
+
+int gru_check(const b200rl_gru_scan_args& a, bool backward) {
+  RL_CHECK_ARG(a.T >= 1 && a.B >= 1 && a.B <= MAXB, "GRU scan supports T >= 1 and batch <= 16 rows per rank");
+  RL_CHECK_ARG(a.R >= 2 && a.R % 2 == 0, "GRU scan supports even recurrent_state_size");
+  // one element of every per-step epilogue per thread (fixed assignments, `Slot`)
+  RL_CHECK_ARG(MAXB * owned_groups(a.R, 0) * 12 <= SCAN_NT, "GRU scan supports recurrent_state_size <= 1024");
+  RL_CHECK_ARG(a.ld_wg >= a.R && a.lat_off >= 0 && a.ld_lat >= a.lat_off + a.R, "GRU scan: leading dimensions too small");
+  RL_CHECK_ARG(sizeof(float) * (size_t)make_geo_g(a.R, 0, backward).total <= 227 * 1024,
+               "weight slice does not fit in shared memory for this model size");
+  return B200RL_OK;
+}
+
+int gru_launch(void* fn, const b200rl_gru_scan_args& a, void** kargs, bool backward, cudaStream_t st) {
+  if (int rc = gru_check(a, backward)) return rc;
+  RL_CHECK_ARG(a.workspace && a.workspace_bytes >= (long long)gru_ws_bytes(a.T, a.B, a.R), "workspace too small");
+  const size_t smem = sizeof(float) * (size_t)make_geo_g(a.R, 0, backward).total;
+  RL_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  // header + LL region are reset; the forward's LayerNorm statistics behind them stay for the backward
+  RL_CUDA(cudaMemsetAsync(a.workspace, 0, WS_HEADER + make_gru_ll(a.R).total * sizeof(u64), st));
+  RL_CUDA(cudaLaunchCooperativeKernel(fn, dim3(SCAN_G), dim3(SCAN_NT), kargs, smem, st));
+  return B200RL_OK;
+}
+
 }  // namespace
 
 extern "C" long long b200rl_rssm_scan_workspace_bytes(int T, int B, int S, int D, int Dx, int R, int Dr) {
@@ -1414,4 +1786,24 @@ extern "C" int b200rl_rssm_scan_profile(const void* workspace, long long* out64,
   RL_CUDA(cudaMemcpyAsync(out64, (const char*)workspace + WS_HEADER, WS_PROF, cudaMemcpyDeviceToHost, st));
   RL_CUDA(cudaStreamSynchronize(st));
   return B200RL_OK;
+}
+
+extern "C" long long b200rl_gru_scan_workspace_bytes(int T, int B, int R) { return (long long)gru_ws_bytes(T, B, R); }
+
+extern "C" int b200rl_gru_scan_check(const b200rl_gru_scan_args* args, int backward) {
+  RL_CHECK_ARG(args, "null args");
+  return gru_check(*args, backward != 0);
+}
+
+extern "C" int b200rl_gru_scan_fwd(const b200rl_gru_scan_args* args, cudaStream_t st) {
+  RL_CHECK_ARG(args, "null args");
+  void* kargs[] = {(void*)args};
+  return gru_launch((void*)gru_scan_fwd_kernel, *args, kargs, false, st);
+}
+
+extern "C" int b200rl_gru_scan_bwd(const b200rl_gru_scan_args* args, const b200rl_gru_scan_grads* grads, cudaStream_t st) {
+  RL_CHECK_ARG(args && grads, "null args");
+  RL_CHECK_ARG(grads->q_g, "q_g (g_pre W_g[:, :R] over all rows) is required");
+  void* kargs[] = {(void*)args, (void*)grads};
+  return gru_launch((void*)gru_scan_bwd_kernel, *args, kargs, true, st);
 }

@@ -77,7 +77,9 @@ def dv3_param_shapes(cfg, actions_dim: Sequence[int], in_channels: int, is_conti
     wm["rssm.recurrent_model.rnn.linear.weight"] = (3 * R, R + dx)
     wm["rssm.recurrent_model.rnn.layer_norm.weight"] = (3 * R,)
     wm["rssm.recurrent_model.rnn.layer_norm.bias"] = (3 * R,)
-    mlp(wm, "rssm.representation_model._model.", R + E + Ev, w.representation_model.hidden_size, 1, Z)
+    # decoupled RSSM: the posterior is a function of the embedding alone (agent.py:1017-1019)
+    mlp(wm, "rssm.representation_model._model.", (0 if w.decoupled_rssm else R) + E + Ev,
+        w.representation_model.hidden_size, 1, Z)
     mlp(wm, "rssm.transition_model._model.", R, w.transition_model.hidden_size, 1, Z)
     if has_cnn:
         wm["observation_model.cnn_decoder.model.0.weight"] = (E, L)
@@ -236,8 +238,7 @@ class DV3Engine:
             raise NotImplementedError(
                 "continuous actions: distribution.type must be auto / scaled_normal — the reference's own train() fails "
                 "with tanh_normal (entropy fallback shape, dreamer_v3.py:294-297) and normal (negative scale)")
-        if w.decoupled_rssm:
-            raise NotImplementedError("decoupled_rssm is not implemented in the B200 engine yet")
+        self.decoupled = bool(w.decoupled_rssm)           # DecoupledRSSM (agent.py:501-593): z_t does not depend on h_t
         _check_supported_modules(cfg)
         if list(a.cnn_keys.encoder) != list(a.cnn_keys.decoder) or list(a.mlp_keys.encoder) != list(a.mlp_keys.decoder):
             raise NotImplementedError("the decoder must reconstruct exactly the encoder's keys")
@@ -264,6 +265,7 @@ class DV3Engine:
         self.S, self.D = w.stochastic_size, w.discrete_size
         self.Z, self.R = self.S * self.D, w.recurrent_model.recurrent_state_size
         self.L = self.Z + self.R
+        self.Rh = 0 if self.decoupled else self.R          # h columns in front of the representation model's input
         self.A = int(sum(self.actions_dim))
         self.du, self.nh = a.dense_units, a.mlp_layers
         self.Dx = w.recurrent_model.dense_units
@@ -454,9 +456,15 @@ class DV3Engine:
         self._graph = None
         # persistent fused RSSM scan (csrc/rssm_scan.cu) when the ops backend has it and the model is inside the kernels'
         # envelope; the backward kernel needs more shared memory than the forward, so it can be refused alone
-        has_scan, dims = hasattr(self.ops, "rssm_scan_fwd"), self._scan_dims()
-        self.fused_scan = has_scan and self.ops.rssm_scan_supported(dims, backward=False)
-        self.fused_scan_bwd = has_scan and self.ops.rssm_scan_supported(dims, backward=True)
+        # (decoupled RSSM: the GRU-only scan kernels of the same file, with their own envelope)
+        if self.decoupled:
+            has_scan, dims = hasattr(self.ops, "gru_scan_fwd"), self._gru_scan_dims()
+            self.fused_scan = has_scan and self.ops.gru_scan_supported(dims, backward=False)
+            self.fused_scan_bwd = has_scan and self.ops.gru_scan_supported(dims, backward=True)
+        else:
+            has_scan, dims = hasattr(self.ops, "rssm_scan_fwd"), self._scan_dims()
+            self.fused_scan = has_scan and self.ops.rssm_scan_supported(dims, backward=False)
+            self.fused_scan_bwd = has_scan and self.ops.rssm_scan_supported(dims, backward=True)
         self._scan_ws = None
         self._scan_q = None
 
@@ -561,7 +569,8 @@ class DV3Engine:
 
         self._encoder_forward()
         # embed part of the representation model's first layer, for all T at once (no recurrence in it)
-        self._project_embedding(self.pe)
+        # (decoupled RSSM: that share is the whole first product)
+        self._project_embedding(self.rp_pre if self.decoupled else self.pe)
         self._scan_forward(first)
         self._decoder_forward()
         rew_logits = self.reward_wm.forward(self.latent)
@@ -644,9 +653,9 @@ class DV3Engine:
         return out
 
     def _project_embedding(self, out: torch.Tensor):
-        """out = embed W_r1[:, R:]^T with embed = [cnn features | vector features] (MultiEncoder, models.py:466-475); the
+        """out = embed W_r1[:, Rh:]^T with embed = [cnn features | vector features] (MultiEncoder, models.py:466-475); the
         two feature blocks stay in their own buffers and meet in this product"""
-        ops, R, E = self.ops, self.R, self.E
+        ops, R, E = self.ops, self.Rh, self.E
         Wr1 = self._w("rssm.representation_model._model.0.weight")
         if self.has_cnn:
             ops.gemm(self.emb, Wr1[:, R:R + E], out, False, True)
@@ -769,7 +778,12 @@ class DV3Engine:
         first-layer weight; given only when z is an exact one-hot sample (imagination), the product becomes a gather.
         `keep`: pre-activations are needed by a backward (x_pre / g_pre / g_ln are written); `h_next`: optional second
         destination of the new h.  Returns True when `h_next` was written."""
-        ops, Z, R = self.ops, self.Z, self.R
+        self._recurrent_input(z, act, x_pre, x_act, win_t, keep)
+        return self._gru_forward(h_prev, x_act, g_pre, g_ln, h_out, hx, h_next, keep)
+
+    def _recurrent_input(self, z, act, x_pre, x_act, win_t=None, keep: bool = True):
+        """x = SiLU(LN(W_in [z, a])) (RecurrentModel.mlp, agent.py:328-341)"""
+        ops, Z = self.ops, self.Z
         p = "rssm.recurrent_model."
         Win = self._w(p + "mlp._model.0.weight")
         fused_x = win_t is not None and ops.onehot_linear_ln_supported(win_t, x_act, x_pre if keep else None)
@@ -784,6 +798,12 @@ class DV3Engine:
         if not fused_x:
             ops.ln_act_fwd(x_pre, self._w(p + "mlp._model.1.weight"), self._w(p + "mlp._model.1.bias"), self.eps,
                            ACT_SILU, x_act)
+
+    def _gru_forward(self, h_prev, x_act, g_pre, g_ln, h_out, hx=None, h_next=None, keep: bool = True):
+        """LayerNormGRUCell (models.py:396-403).  `x_act` None: g_pre already holds x's share of the product (decoupled
+        RSSM: x is known for every step up front), h's share is added to it."""
+        ops, R = self.ops, self.R
+        p = "rssm.recurrent_model."
         Wg = self._w(p + "rnn.linear.weight")
         if hx is not None and hx.shape[0] <= FUSED_DENSE_MAX_ROWS and ops.gemm_ln_supported(hx, Wg, 1):
             # product + split-K sum + LayerNorm + gate in two launches; the new h also lands in `h_next` (the next
@@ -794,8 +814,9 @@ class DV3Engine:
         if hx is not None:                                   # [h | x] contiguous (x_act is its right half)
             ops.gemm(hx, Wg, g_pre, False, True)
         else:
-            ops.gemm(h_prev, Wg[:, :R], g_pre, False, True)
-            ops.gemm(x_act, Wg[:, R:], g_pre, False, True, accumulate=True)
+            ops.gemm(h_prev, Wg[:, :R], g_pre, False, True, accumulate=x_act is None)
+            if x_act is not None:
+                ops.gemm(x_act, Wg[:, R:], g_pre, False, True, accumulate=True)
         ops.ln_act_fwd(g_pre, self._w(p + "rnn.layer_norm.weight"), self._w(p + "rnn.layer_norm.bias"), self.eps,
                        ACT_NONE, g_ln)
         ops.gru_gate_fwd(g_ln, h_prev, h_out)
@@ -809,16 +830,22 @@ class DV3Engine:
         ops, Z, R = self.ops, self.Z, self.R
         p = "rssm.recurrent_model."
         Win, Wg = self._w(p + "mlp._model.0.weight"), self._w(p + "rnn.linear.weight")
-        ops.gru_gate_bwd(g_ln, h_prev, dh, d_g_ln, dh_prev)
-        ops.ln_act_bwd(g_pre, self._w(p + "rnn.layer_norm.weight"), self._w(p + "rnn.layer_norm.bias"), self.eps, ACT_NONE,
-                       d_g_ln, d_g_pre, None, None)
-        ops.gemm(d_g_pre, Wg[:, :R], dh_prev, False, False, accumulate=True)
+        self._gru_backward(g_ln, h_prev, g_pre, dh, d_g_ln, d_g_pre, dh_prev)
         ops.gemm(d_g_pre, Wg[:, R:], d_x_act, False, False)
         ops.ln_act_bwd(x_pre, self._w(p + "mlp._model.1.weight"), self._w(p + "mlp._model.1.bias"), self.eps, ACT_SILU,
                        d_x_act, d_x_pre, None, None)
         ops.gemm(d_x_pre, Win[:, :Z], dz, False, False)
         if da is not None:
             ops.gemm(d_x_pre, Win[:, Z:], da, False, False)
+
+    def _gru_backward(self, g_ln, h_prev, g_pre, dh, d_g_ln, d_g_pre, dh_prev):
+        """Data-gradient backward of `_gru_forward` with respect to h_prev: dh -> d_g_ln, d_g_pre, dh_prev"""
+        ops = self.ops
+        p = "rssm.recurrent_model.rnn."
+        ops.gru_gate_bwd(g_ln, h_prev, dh, d_g_ln, dh_prev)
+        ops.ln_act_bwd(g_pre, self._w(p + "layer_norm.weight"), self._w(p + "layer_norm.bias"), self.eps, ACT_NONE,
+                       d_g_ln, d_g_pre, None, None)
+        ops.gemm(d_g_pre, self._w(p + "linear.weight")[:, :self.R], dh_prev, False, False, accumulate=True)
 
     def _transition_forward(self, h, tr_pre, tr_act, raw, keep: bool = True):
         ops = self.ops
@@ -841,10 +868,12 @@ class DV3Engine:
 
     def _posterior_forward(self, h, rp_pre, rp_act, raw, noise, z_out, mix_out=None):
         """Representation model on [h | embed] and its sample z_out (agent.py:451-465).  `rp_pre` holds the embedding's
-        share of the first product on entry (`_project_embedding`); h's share is added to it."""
+        share of the first product on entry (`_project_embedding`); h's share is added to it (decoupled RSSM,
+        agent.py:582-593: there is none and `h` is None)."""
         ops, R = self.ops, self.R
         pr = "rssm.representation_model._model."
-        ops.gemm(h, self._w(pr + "0.weight")[:, :R], rp_pre, False, True, accumulate=True)
+        if h is not None:
+            ops.gemm(h, self._w(pr + "0.weight")[:, :R], rp_pre, False, True, accumulate=True)
         ops.ln_act_fwd(rp_pre, self._w(pr + "1.weight"), self._w(pr + "1.bias"), self.eps, ACT_SILU, rp_act)
         ops.gemm(rp_act, self._w(pr + "3.weight"), raw, False, True, bias=self._w(pr + "3.bias"))
         ops.cat_sample(raw, noise, self.unimix, self.S, self.D, z_out, mix_out)
@@ -857,9 +886,11 @@ class DV3Engine:
         ops.tanh_fwd(self._w("rssm.initial_recurrent_state").view(1, R), self.h0)
         self._transition_forward(self.h0, self.init_tr_pre, self.init_tr_act, self.init_raw)
         ops.cat_sample(self.init_raw, None, self.unimix, self.S, self.D, self.z0)
-        if self.fused_scan:
+        if self.decoupled:
+            self._scan_forward_decoupled(first)
+        elif self.fused_scan:
             self._scan_forward_fused(first)
-        for t in (() if self.fused_scan else range(self.T)):
+        for t in (() if self.fused_scan or self.decoupled else range(self.T)):
             s = slice(t * B, (t + 1) * B)
             f = first[s]
             if t == 0:
@@ -878,6 +909,39 @@ class DV3Engine:
                                     self.latent[s, :Z], self.post_mix[s])
         self._prior_forward()
 
+    def _scan_forward_decoupled(self, first: torch.Tensor):
+        """DecoupledRSSM (dreamer_v3.py:115-129, agent.py:571-593): the posterior is a function of the embedding alone, so
+        z of every step, x = SiLU(LN(W_in [z_{t-1}, a_{t-1}])) and x's share of the GRU product are batched over all
+        T*B rows; only h_in W_g[:, :R]^T, the GRU LayerNorm and the gate stay on the recurrence."""
+        ops, B, N, Z, R = self.ops, self.B, self.N, self.Z, self.R
+        self._posterior_forward(None, self.rp_pre, self.rp_act, self.post_raw, self.noise_post.view(N, Z),
+                                self.latent[:, :Z], self.post_mix)
+        ops.mask_mix(self.zero_z, self.z0, first[:B], self.z_in[:B])
+        if N > B:
+            ops.mask_mix(self.latent[:N - B, :Z], self.z0, first[B:], self.z_in[B:])
+        ops.mask_rows(self.shift_actions, first, self.a_in)
+        self._recurrent_input(self.z_in, self.a_in, self.x_pre, self.x_act)
+        ops.gemm(self.x_act, self._w("rssm.recurrent_model.rnn.linear.weight")[:, R:], self.g_pre, False, True)
+        if self.fused_scan:
+            if self._scan_ws is None:
+                self._scan_ws = ops.gru_scan_workspace(self.T, B, R)
+            ops.gru_scan_fwd(self._gru_scan_dims(), self.eps, self._gru_scan_tensors(first), self._scan_ws)
+            return
+        for t in range(self.T):
+            s = slice(t * B, (t + 1) * B)
+            hp = self.zero_h if t == 0 else self.latent[(t - 1) * B:t * B, Z:]
+            ops.mask_mix(hp, self.h0, first[s], self.h_in[s])
+            self._gru_forward(self.h_in[s], None, self.g_pre[s], self.g_ln[s], self.latent[s, Z:])
+
+    def _gru_scan_dims(self):
+        return dict(T=self.T, B=self.B, R=self.R, ld_wg=self.R + self.Dx, ld_lat=self.L, lat_off=self.Z)
+
+    def _gru_scan_tensors(self, first: torch.Tensor):
+        p = "rssm.recurrent_model.rnn."
+        return dict(W_g=self._w(p + "linear.weight"), lng_g=self._w(p + "layer_norm.weight"),
+                    lng_b=self._w(p + "layer_norm.bias"), h0=self.h0, first=first, g_pre=self.g_pre, g_ln=self.g_ln,
+                    h_in=self.h_in, latent=self.latent)
+
     def _prior_forward(self):
         """The prior of every step (transition model on h_t, agent.py:433) is off the recurrence: with the h sequence
         finished it is two batched tensor-core products over all T*B rows instead of 2 x T skinny ones in the scan."""
@@ -895,7 +959,7 @@ class DV3Engine:
 
     def _scan_dims(self):
         return dict(T=self.T, B=self.B, S=self.S, D=self.D, R=self.R, A=self.A, Dx=self.Dx, Dt=self.Dt, Dr=self.Dr,
-                    ld_lat=self.L, ld_wr1=self.R + self.E + self.Ev)
+                    ld_lat=self.L, ld_wr1=self.Rh + self.E + self.Ev)
 
     def _scan_tensors(self, first: torch.Tensor):
         p = "rssm.recurrent_model."
@@ -944,7 +1008,6 @@ class DV3Engine:
         """BPTT over the scan (SURVEY.md App. E): the batched prior backward, then the posterior recurrence.  Per step
         only the data-gradient GEMMs run; the weight gradients are single big GEMMs over all T*B rows afterwards."""
         ops, B, Z, R = self.ops, self.B, self.Z, self.R
-        p = "rssm.recurrent_model."
         pt, pr = "rssm.transition_model._model.", "rssm.representation_model._model."
         Wr1 = self._w(pr + "0.weight")
         ops.zero(self.dz_carry)
@@ -952,9 +1015,11 @@ class DV3Engine:
         ops.zero(self.d_h0)
         self._prior_backward()
         fused = self.fused_scan and self.fused_scan_bwd
-        if fused:
+        if self.decoupled:
+            self._scan_backward_decoupled(first, fused)
+        elif fused:
             self._scan_backward_fused(first)
-        for t in (() if fused else reversed(range(self.T))):
+        for t in (() if fused or self.decoupled else reversed(range(self.T))):
             s = slice(t * B, (t + 1) * B)
             f = first[s]
             ops.copy(self.d_latent[s, :Z], self.dz_tot)
@@ -974,10 +1039,25 @@ class DV3Engine:
             ops.mask_bwd(self.dz_in, f, self.dz_carry, None)
             ops.mask_bwd(self.dh_in, f, self.dh_carry, self.d_h0)
         # ---- deferred parameter gradients over all N rows
-        N = self.N
-        h_all = self.latent[:, Z:]
-        gW = self._gw
-        # representation model
+        self._representation_param_grads()
+        gW, h_all = self._gw, self.latent[:, Z:]
+        # transition model
+        ops.gemm(self.d_prior_raw, self.tr_act, gW(pt + "3.weight"), True, False)
+        ops.col_sum(self.d_prior_raw, gW(pt + "3.bias"))
+        ops.gemm(self.d_tr_pre, h_all, gW(pt + "0.weight"), True, False)
+        if not self.decoupled:          # (decoupled: done in front of the posterior's backward, which consumes d_x_pre)
+            self._recurrent_param_grads()
+        # learned initial recurrent state: h0 = tanh(param)
+        if self.cfg.algo.world_model.get("learnable_initial_recurrent_state", True):
+            ops.tanh_bwd(self.h0.view(R), self.d_h0, gW("rssm.initial_recurrent_state"))
+        # else: a buffer in the reference (agent.py:382-389) — its gradient stays at the zero `wm.grad` was reset to, the
+        # norm ignores it and Adam's zero moments leave the value untouched
+
+    def _representation_param_grads(self):
+        """Parameter gradients of the representation model over all N rows, and the gradient of the embedding"""
+        ops, R, E, Z, gW = self.ops, self.Rh, self.E, self.Z, self._gw
+        pr = "rssm.representation_model._model."
+        Wr1 = self._w(pr + "0.weight")
         ops.gemm(self.d_post_raw, self.rp_act, gW(pr + "3.weight"), True, False)
         ops.col_sum(self.d_post_raw, gW(pr + "3.bias"))
         # LayerNorm parameter gradients over all rows; the same pass (re)writes the pre-activation gradients the weight
@@ -985,36 +1065,65 @@ class DV3Engine:
         ops.ln_act_bwd(self.rp_pre, self._w(pr + "1.weight"), self._w(pr + "1.bias"), self.eps, ACT_SILU,
                        self.d_rp_act, self.d_rp_pre, gW(pr + "1.weight"), gW(pr + "1.bias"))
         gWr1 = gW(pr + "0.weight")
-        ops.gemm(self.d_rp_pre, h_all, gWr1[:, :R], True, False)
-        E = self.E
+        if R:
+            ops.gemm(self.d_rp_pre, self.latent[:, Z:], gWr1[:, :R], True, False)
         if self.has_cnn:
             ops.gemm(self.d_rp_pre, self.emb, gWr1[:, R:R + E], True, False)
             ops.gemm(self.d_rp_pre, Wr1[:, R:R + E], self.d_emb, False, False)
         if self.vec_keys:
             ops.gemm(self.d_rp_pre, self.venc.act[-1], gWr1[:, R + E:], True, False)
             ops.gemm(self.d_rp_pre, Wr1[:, R + E:], self.d_emb_vec, False, False)
-        # transition model
-        ops.gemm(self.d_prior_raw, self.tr_act, gW(pt + "3.weight"), True, False)
-        ops.col_sum(self.d_prior_raw, gW(pt + "3.bias"))
-        ops.gemm(self.d_tr_pre, h_all, gW(pt + "0.weight"), True, False)
-        # recurrent model
+
+    def _recurrent_param_grads(self, x_data_grad: bool = False):
+        """Parameter gradients of the recurrent model over all N rows.  `x_data_grad`: d_x_act is not there yet and is
+        one batched product of d_g_pre (decoupled RSSM: x is off the recurrence)."""
+        ops, Z, R, gW = self.ops, self.Z, self.R, self._gw
+        p = "rssm.recurrent_model."
         ops.ln_act_bwd(self.g_pre, self._w(p + "rnn.layer_norm.weight"), self._w(p + "rnn.layer_norm.bias"),
                        self.eps, ACT_NONE, self.d_g_ln, self.d_g_pre, gW(p + "rnn.layer_norm.weight"),
                        gW(p + "rnn.layer_norm.bias"))
         gWg = gW(p + "rnn.linear.weight")
         ops.gemm(self.d_g_pre, self.h_in, gWg[:, :R], True, False)
         ops.gemm(self.d_g_pre, self.x_act, gWg[:, R:], True, False)
+        if x_data_grad:
+            ops.gemm(self.d_g_pre, self._w(p + "rnn.linear.weight")[:, R:], self.d_x_act, False, False)
         ops.ln_act_bwd(self.x_pre, self._w(p + "mlp._model.1.weight"), self._w(p + "mlp._model.1.bias"), self.eps,
                        ACT_SILU, self.d_x_act, self.d_x_pre, gW(p + "mlp._model.1.weight"),
                        gW(p + "mlp._model.1.bias"))
         gWin = gW(p + "mlp._model.0.weight")
         ops.gemm(self.d_x_pre, self.z_in, gWin[:, :Z], True, False)
         ops.gemm(self.d_x_pre, self.a_in, gWin[:, Z:], True, False)
-        # learned initial recurrent state: h0 = tanh(param)
-        if self.cfg.algo.world_model.get("learnable_initial_recurrent_state", True):
-            ops.tanh_bwd(self.h0.view(R), self.d_h0, gW("rssm.initial_recurrent_state"))
-        # else: a buffer in the reference (agent.py:382-389) — its gradient stays at the zero `wm.grad` was reset to, the
-        # norm ignores it and Adam's zero moments leave the value untouched
+
+    def _scan_backward_decoupled(self, first: torch.Tensor, fused: bool):
+        """BPTT of the decoupled scan: the GRU recurrence alone walks back through time (one persistent kernel inside
+        its envelope, else per step); x, z_{t-1} and the posterior are batched over all T*B rows behind it."""
+        ops, B, N, Z, R = self.ops, self.B, self.N, self.Z, self.R
+        p, pr = "rssm.recurrent_model.", "rssm.representation_model._model."
+        if fused:
+            if self._scan_q is None:
+                self._scan_q = torch.zeros(N, R, dtype=torch.float32, device=self.device)
+            # g_pre W_g[:, :R]: lets the kernel apply the LayerNorm-backward correction on the consumer side
+            ops.gemm(self.g_pre, self._w(p + "rnn.linear.weight")[:, :R], self._scan_q, False, False)
+            ops.gru_scan_bwd(self._gru_scan_dims(), self.eps, self._gru_scan_tensors(first),
+                             dict(d_latent=self.d_latent, d_g_ln=self.d_g_ln, d_h0=self.d_h0, q_g=self._scan_q),
+                             self._scan_ws)
+        for t in (() if fused else reversed(range(self.T))):
+            s = slice(t * B, (t + 1) * B)
+            ops.copy(self.d_latent[s, Z:], self.dh_tot)
+            ops.axpy(self.dh_carry, self.dh_tot)
+            self._gru_backward(self.g_ln[s], self.h_in[s], self.g_pre[s], self.dh_tot, self.d_g_ln[s], self.d_g_pre[s],
+                               self.dh_in)
+            ops.mask_bwd(self.dh_in, first[s], self.dh_carry, self.d_h0)
+        self._recurrent_param_grads(x_data_grad=True)
+        # z_{t-1} feeds x_t: (1 - f_t) d_x_pre[t] W_in[:, :Z] joins the gradient of z_{t-1} (the f_t share goes to z0, a
+        # mode: no gradient); d_x_act has been consumed and stages the masked rows
+        if N > B:
+            ops.mask_rows(self.d_x_pre, first, self.d_x_act)
+            ops.gemm(self.d_x_act[B:], self._w(p + "mlp._model.0.weight")[:, :Z], self.d_latent[:N - B, :Z], False, False,
+                     accumulate=True)
+        ops.cat_sample_bwd(self.post_raw, self.d_latent[:, :Z], self.d_post_mix, self.unimix, self.S, self.D,
+                           self.d_post_raw)
+        ops.gemm(self.d_post_raw, self._w(pr + "3.weight"), self.d_rp_act, False, False)
 
     # ------------------------------------------------------------------ optimiser
     def _wm_buckets(self):

@@ -138,6 +138,8 @@ def _struct(name: str, typedef: str, exclude=()):
 
 RssmScanArgs = _struct("RssmScanArgs", "b200rl_rssm_scan_args", exclude=("workspace",))   # passed on its own
 RssmScanGrads = _struct("RssmScanGrads", "b200rl_rssm_scan_grads")
+GruScanArgs = _struct("GruScanArgs", "b200rl_gru_scan_args", exclude=("workspace",))
+GruScanGrads = _struct("GruScanGrads", "b200rl_gru_scan_grads")
 
 
 class CudaOps:
@@ -562,6 +564,48 @@ class CudaOps:
         out = (ctypes.c_longlong * 64)()
         self._ck(self.lib.b200rl_rssm_scan_profile(_p(workspace), out, self._st()), 0)
         return [list(out[:32]), list(out[32:])]
+
+    # ------------------------------------------------------------------ persistent GRU-only scan (decoupled RSSM)
+    def gru_scan_workspace(self, T: int, B: int, R: int) -> torch.Tensor:
+        n = self.lib.b200rl_gru_scan_workspace_bytes(T, B, R)
+        return torch.zeros((n + 3) // 4, dtype=torch.int32, device=self.device)
+
+    @staticmethod
+    def _gru_scan_dims(dims: dict) -> GruScanArgs:
+        return GruScanArgs(**{k: int(dims[k]) for k, t in GruScanArgs._fields_ if t is ctypes.c_int})
+
+    def _gru_scan_args(self, dims: dict, eps: float, tensors: dict, workspace: torch.Tensor) -> GruScanArgs:
+        a = self._gru_scan_dims(dims)
+        a.eps = float(eps)
+        for name in GruScanArgs.POINTERS:
+            t = tensors[name]
+            assert t.is_cuda and t.dtype == torch.float32, name
+            assert name in ("W_g", "latent") or t.is_contiguous(), name     # those two carry their leading dimension
+            setattr(a, name, t.data_ptr())
+        assert _ld(tensors["W_g"]) == a.ld_wg and _ld(tensors["latent"]) == a.ld_lat
+        a.workspace, a.workspace_bytes = workspace.data_ptr(), workspace.numel() * workspace.element_size()
+        return a
+
+    def gru_scan_supported(self, dims: dict, backward: bool) -> bool:
+        """whether the forward / backward kernel runs these dims (the int fields of `b200rl_gru_scan_args`); launches
+        nothing"""
+        return self.lib.b200rl_gru_scan_check(ctypes.byref(self._gru_scan_dims(dims)), int(backward)) == 0
+
+    def gru_scan_fwd(self, dims: dict, eps: float, tensors: dict, workspace: torch.Tensor):
+        """tensors: name -> device tensor for every pointer field but the workspace (GruScanArgs.POINTERS)"""
+        a = self._gru_scan_args(dims, eps, tensors, workspace)
+        self._ck(self.lib.b200rl_gru_scan_fwd(ctypes.byref(a), self._st()))
+
+    def gru_scan_bwd(self, dims: dict, eps: float, tensors: dict, grads: dict, workspace: torch.Tensor):
+        a = self._gru_scan_args(dims, eps, tensors, workspace)
+        q = GruScanGrads()
+        for name in GruScanGrads.POINTERS:
+            t = grads[name]
+            assert t.is_cuda and t.dtype == torch.float32, name
+            assert name == "d_latent" or t.is_contiguous(), name
+            setattr(q, name, t.data_ptr())
+        assert _ld(grads["d_latent"]) == a.ld_lat
+        self._ck(self.lib.b200rl_gru_scan_bwd(ctypes.byref(a), ctypes.byref(q), self._st()))
 
     # ------------------------------------------------------------------ replay / PPO
     def replay_gather(self, storage, idx, out, n_samples: int, batch: int, seq_len: int):
