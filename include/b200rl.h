@@ -85,7 +85,14 @@ int b200rl_gemm_ln_presplit(const float* A, const float* Whi, const float* Wlo, 
                             long long ldho, float* h_out2, long long ldho2, cudaStream_t stream);
 /* nn.LayerNorm(eps) (+ nn.SiLU): miniblock sheeprl/utils/model.py:34-88; LayerNormChannelLast
  * sheeprl/models/models.py:507-518 (channel-last is native here).  act: 0 none, 1 SiLU, 2 tanh, 3 ReLU (the last two:
- * PPO MLPs with layer_norm=True, sheeprl/algos/ppo/agent.py:58-66,152-176). */
+ * PPO MLPs with layer_norm=True, sheeprl/algos/ppo/agent.py:58-66,152-176).
+ * `_route` is the kernel both launches pick for C channels, row strides ld0..ld2 and row bases p0..p2 (forward: X, Y,
+ * ld2 = 0, p2 = NULL; backward: X, dY, dX), from the values alone: 0 the warp-per-row kernels (any C; the backward
+ * refuses C > 28000), 1 the register-resident rows (C in {32, 48, 64, 96, 128, 192, 256, 384, 512, 640, 768, 1024,
+ * 1536}), 2 one CTA per row (C % 4 == 0, 1536 < C <= 16384); 1 and 2 need row strides that are multiples of 4 floats
+ * and 16-byte aligned p0..p2, gamma and beta. */
+int b200rl_ln_act_route(int C, long long ld0, long long ld1, long long ld2, const float* p0, const float* p1,
+                        const float* p2, const float* gamma, const float* beta);
 int b200rl_ln_act_fwd(const float* X, const float* gamma, const float* beta, float* Y, long long M, int C,
                       long long ldx, long long ldy, float eps, int act, cudaStream_t stream);
 int b200rl_ln_act_bwd(const float* X, const float* gamma, const float* beta, const float* dY, float* dX, float* dgamma,

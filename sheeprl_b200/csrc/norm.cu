@@ -509,7 +509,16 @@ int grid_for_rows(long long M) {
   return (int)blocks;
 }
 
+constexpr int ROUTE_GENERIC = 0, ROUTE_VEC = 1, ROUTE_WIDE = 2;
+
 }  // namespace
+
+extern "C" int b200rl_ln_act_route(int C, long long ld0, long long ld1, long long ld2, const float* p0, const float* p1,
+                                   const float* p2, const float* gamma, const float* beta) {
+  if (vec_ok(C, ld0, ld1, ld2, p0, p1, p2, gamma, beta)) return ROUTE_VEC;
+  if (wide_ok(C, ld0, ld1, ld2, p0, p1, p2, gamma, beta)) return ROUTE_WIDE;
+  return ROUTE_GENERIC;
+}
 
 extern "C" int b200rl_ln_act_fwd(const float* X, const float* gamma, const float* beta, float* Y, long long M, int C,
                                  long long ldx, long long ldy, float eps, int act, cudaStream_t st) {
@@ -517,7 +526,8 @@ extern "C" int b200rl_ln_act_fwd(const float* X, const float* gamma, const float
   RL_CHECK_ARG(C > 0 && ldx >= C && ldy >= C, "bad C / ld");
   RL_CHECK_ARG(act >= ACT_NONE && act <= ACT_RELU, "act must be 0 (none), 1 (SiLU), 2 (tanh) or 3 (ReLU)");
   if (M <= 0) return B200RL_OK;
-  if (vec_ok(C, ldx, ldy, 0, X, Y, nullptr, gamma, beta)) {
+  const int route = b200rl_ln_act_route(C, ldx, ldy, 0, X, Y, nullptr, gamma, beta);
+  if (route == ROUTE_VEC) {
 #define LN_FWD_VEC(LPR_, NV_) \
   ln_act_fwd_vec_kernel<LPR_, NV_><<<vec_grid(M, 32 / LPR_), 256, 0, st>>>(X, gamma, beta, Y, M, ldx, ldy, eps, act)
     switch (C) {
@@ -539,7 +549,7 @@ extern "C" int b200rl_ln_act_fwd(const float* X, const float* gamma, const float
     RL_CHECK_LAUNCH();
     return B200RL_OK;
   }
-  if (wide_ok(C, ldx, ldy, 0, X, Y, nullptr, gamma, beta)) {
+  if (route == ROUTE_WIDE) {
     const int grid = (int)(M < 4LL * kNumSMs ? M : 4LL * kNumSMs);
     ln_act_fwd_wide_kernel<<<grid, WIDE_NT, 0, st>>>(X, gamma, beta, Y, M, C, ldx, ldy, eps, act);
     RL_CHECK_LAUNCH();
@@ -557,12 +567,15 @@ extern "C" int b200rl_ln_act_bwd(const float* X, const float* gamma, const float
   RL_CHECK_ARG((dgamma == nullptr) == (dbeta == nullptr), "dgamma/dbeta must both be given or both be null");
   RL_CHECK_ARG(C > 0 && ldx >= C && lddy >= C && lddx >= C, "bad C / ld");
   RL_CHECK_ARG(act >= ACT_NONE && act <= ACT_RELU, "act must be 0 (none), 1 (SiLU), 2 (tanh) or 3 (ReLU)");
+  const int route = b200rl_ln_act_route(C, ldx, lddy, lddx, X, dY, dX, gamma, beta);
+  // every refusal comes before the first write: a refused call leaves dgamma / dbeta as the caller had them
+  RL_CHECK_ARG(route != ROUTE_GENERIC || C <= 28000, "C too large for the shared accumulator path");
   if (dgamma && !accumulate) {
     RL_CUDA(cudaMemsetAsync(dgamma, 0, sizeof(float) * C, st));
     RL_CUDA(cudaMemsetAsync(dbeta, 0, sizeof(float) * C, st));
   }
   if (M <= 0) return B200RL_OK;
-  if (vec_ok(C, ldx, lddy, lddx, X, dY, dX, gamma, beta)) {
+  if (route == ROUTE_VEC) {
     // every CTA ends with 2*C global atomics into dgamma / dbeta: for wide rows (a warp already keeps >= 2 KB in flight) two
     // CTAs per SM saturate HBM and cut that traffic 4x (ncu: [16384,512] ran at 0.34 of the HBM peak with 1184 CTAs)
     const int bwd_cap = (dgamma && C >= 256) ? 2 * kNumSMs : (1 << 30);
@@ -588,7 +601,7 @@ extern "C" int b200rl_ln_act_bwd(const float* X, const float* gamma, const float
     RL_CHECK_LAUNCH();
     return B200RL_OK;
   }
-  if (wide_ok(C, ldx, lddy, lddx, X, dY, dX, gamma, beta)) {
+  if (route == ROUTE_WIDE) {
     const int wgrid = (int)(M < 2LL * kNumSMs ? M : 2LL * kNumSMs);
     ln_act_bwd_wide_kernel<<<wgrid, WIDE_NT, 0, st>>>(X, gamma, beta, dY, dX, dgamma, dbeta, M, C, ldx, lddy, lddx, eps, act);
     RL_CHECK_LAUNCH();
@@ -606,7 +619,7 @@ extern "C" int b200rl_ln_act_bwd(const float* X, const float* gamma, const float
   else if (C <= 512) LN_BWD(16, 0);
   else {
     // wide rows (XL: the GRU's joint LayerNorm spans 3*4096 channels): per-CTA gamma/beta partials in opted-in smem
-    RL_CHECK_ARG(C <= 28000, "C too large for the shared accumulator path");
+    // (C <= 28000, checked above)
     const size_t smem = sizeof(float) * 2 * (size_t)C;
     if (smem > 48 * 1024)
       RL_CUDA(cudaFuncSetAttribute(ln_act_bwd_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -554,7 +554,7 @@ extern "C" int b200rl_onehot_linear_ln_supported(const float* WT, const float* g
 
 extern "C" int b200rl_onehot_linear(const float* z, const float* act, const float* WT, float* out, long long M, int S,
                                     int K, int A, int N, long long ldz, long long lda, long long ldo, cudaStream_t st) {
-  RL_CHECK_ARG(z && act && WT && out, "null pointer");
+  RL_CHECK_ARG(z && (act || A == 0) && WT && out, "null pointer");   // act is read only for A > 0 action columns
   RL_CHECK_ARG(b200rl_onehot_linear_supported(S, K, A, N), "bad dims (S <= 64 groups, A <= 32)");
   if (M <= 0) return B200RL_OK;
   onehot_linear_kernel<<<(unsigned)M, 256, 0, st>>>(z, act, WT, out, S, K, A, N, ldz, lda, ldo, nullptr, nullptr, 0.f, nullptr, 0);
@@ -566,7 +566,7 @@ extern "C" int b200rl_onehot_linear_ln(const float* z, const float* act, const f
                                        const float* beta, float eps, float* pre, long long ldpre, float* out, long long M,
                                        int S, int K, int A, int N, long long ldz, long long lda, long long ldo,
                                        cudaStream_t st) {
-  RL_CHECK_ARG(z && act && WT && out && gamma && beta, "null pointer");
+  RL_CHECK_ARG(z && (act || A == 0) && WT && out && gamma && beta, "null pointer");
   RL_CHECK_ARG(b200rl_onehot_linear_supported(S, K, A, N), "bad dims (S <= 64 groups, A <= 32)");
   RL_CHECK_ARG(b200rl_onehot_linear_ln_supported(WT, gamma, beta, out, pre, N, ldo, ldpre),
                "onehot_linear_ln: N a multiple of 128 up to 1024, 16-byte aligned rows");

@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 import torch
 
+from oracle import ln_ref
 from oracle.ops_emul import EmulOps
 from tests.test_lib_cpu import HEAD_SAMPLE, ONEHOT_LINEAR, WGRAD_TC
 
@@ -38,6 +39,22 @@ def run_both(ops, name, tensors, *scalars, outputs, **kw):
     cpu = {k: (v.clone() if v is not None else None) for k, v in tensors.items()}
     gpu = {k: (v.clone().cuda() if v is not None else None) for k, v in tensors.items()}
     return cu, em, cpu, gpu
+
+
+def ln_close(X, gam, bet, eps, act, dY, got, want):
+    """LayerNorm kernel vs emulator: |kernel - emulator| <= the sum of both float64 error bounds (oracle/ln_ref.py),
+    element by element for y and dX, column by column for dgamma / dbeta.  got / want: (y, dX, dgamma, dbeta).  A
+    tolerance relative to the largest entry was marginal: the float64 reference puts the kernel at the once-failed shape
+    (tanh, M = 1000, C = 32, eps 1e-5) at 0.28 of its bound and the emulator within half of it."""
+    M = X.shape[0]
+    y64 = ln_ref.ln_act_fwd64(X, gam, bet, eps, act)[0]
+    b_dx, p_g, p_b = ln_ref.ln_act_bwd_bound(X, gam, bet, eps, act, dY)
+    mag = ln_ref.ln_act_bwd64(X, gam, bet, eps, act, dY)[3]
+    bounds = (ln_ref.ln_act_fwd_bound(X, gam, bet, eps, act, y64), b_dx, ln_ref.param_bound(M, mag["dgamma"], p_g),
+              ln_ref.param_bound(M, mag["dbeta"], p_b))
+    for name, g_, w_, b_ in zip(("ln fwd", "ln dX", "ln dgamma", "ln dbeta"), got, want, bounds):
+        err = (g_.detach().cpu().double() - w_.double()).abs()
+        assert bool((err <= 2 * b_).all()), (name, float((err / b_).max()))
 
 
 GEMM_SHAPES = [
@@ -189,18 +206,15 @@ def test_ln_act(ops, M, C, act):
     Yg = torch.empty(M, C, device="cuda")
     em.ln_act_fwd(X, gam, bet, 1e-3, act, Yc)
     cu.ln_act_fwd(X.cuda(), gam.cuda(), bet.cuda(), 1e-3, act, Yg)
-    close(Yg, Yc, what="ln fwd")
     dXc, dgc, dbc = torch.empty(M, C), torch.empty(C), torch.empty(C)
     dXg, dgg, dbg = torch.empty(M, C, device="cuda"), torch.empty(C, device="cuda"), torch.empty(C, device="cuda")
     em.ln_act_bwd(X, gam, bet, 1e-3, act, dY, dXc, dgc, dbc)
     cu.ln_act_bwd(X.cuda(), gam.cuda(), bet.cuda(), 1e-3, act, dY.cuda(), dXg, dgg, dbg)
-    close(dXg, dXc, rtol=2e-5, what="ln dX")
-    close(dgg, dgc, rtol=2e-5 * max(M, 16) ** 0.5 / 4, what="ln dgamma")
-    close(dbg, dbc, rtol=2e-5 * max(M, 16) ** 0.5 / 4, what="ln dbeta")
+    ln_close(X, gam, bet, 1e-3, act, dY, (Yg, dXg, dgg, dbg), (Yc, dXc, dgc, dbc))
     # in-place (dX aliases dY), no parameter grads
     dYg = dY.cuda()
     cu.ln_act_bwd(X.cuda(), gam.cuda(), bet.cuda(), 1e-3, act, dYg, dYg, None, None)
-    close(dYg, dXc, rtol=2e-5, what="ln dX in place")
+    ln_close(X, gam, bet, 1e-3, act, dY, (Yg, dYg, dgg, dbg), (Yc, dXc, dgc, dbc))
 
 
 @pytest.mark.parametrize("M,C", [(1000, 32), (37, 72), (64, 64), (16, 1536), (256, 24)])
@@ -217,14 +231,11 @@ def test_ln_act_tanh_relu(ops, M, C, act):
     Yc, Yg = torch.empty(M, C), torch.empty(M, C, device="cuda")
     em.ln_act_fwd(X, gam, bet, 1e-5, act, Yc)
     cu.ln_act_fwd(X.cuda(), gam.cuda(), bet.cuda(), 1e-5, act, Yg)
-    close(Yg, Yc, what="ln fwd")
     dXc, dgc, dbc = torch.empty(M, C), torch.empty(C), torch.empty(C)
     dXg, dgg, dbg = torch.empty(M, C, device="cuda"), torch.empty(C, device="cuda"), torch.empty(C, device="cuda")
     em.ln_act_bwd(X, gam, bet, 1e-5, act, dY, dXc, dgc, dbc)
     cu.ln_act_bwd(X.cuda(), gam.cuda(), bet.cuda(), 1e-5, act, dY.cuda(), dXg, dgg, dbg)
-    close(dXg, dXc, rtol=2e-5, what="ln dX")
-    close(dgg, dgc, rtol=2e-5 * max(M, 16) ** 0.5 / 4, what="ln dgamma")
-    close(dbg, dbc, rtol=2e-5 * max(M, 16) ** 0.5 / 4, what="ln dbeta")
+    ln_close(X, gam, bet, 1e-5, act, dY, (Yg, dXg, dgg, dbg), (Yc, dXc, dgc, dbc))
 
 
 @pytest.mark.parametrize("M,C", [(1024, 255), (1048576 // 64, 3), (17, 4096), (3, 1),

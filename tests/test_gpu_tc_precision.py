@@ -24,6 +24,7 @@ import pytest
 import torch
 
 from oracle import tc_ref
+from oracle.ln_ref import ln_bound
 
 pytestmark = pytest.mark.gpu
 
@@ -197,23 +198,6 @@ def test_gemm_tc_epilogue_precision(cu, route, epi, odd_ldc):
 
 
 # ------------------------------------------------------------------------------------ fused product + LayerNorm
-def ln_bound(pre64, mag, gamma, beta, tau):
-    """Per-element bound on |LN(pre) - LN64(pre64)| with LN(x) = (x - mu) rstd gamma + beta.
-
-    The sum over j of |d LN_i / d x_j| is at most rstd |gamma_i| (2 + |xhat_i|), so an input error of at most D per row
-    moves LN_i by at most rstd |gamma_i| (2 + |xhat_i|) D.  D is the product bound tau * sum|a||b| plus the fp32
-    LayerNorm arithmetic seen as an input perturbation: mean and variance summed over N in fp32, (log2 N + 4) u max|x|.
-    Storing the result adds 4 u (|LN_i| + |beta_i|)."""
-    N = pre64.shape[1]
-    mu = pre64.mean(1, keepdim=True)
-    var = ((pre64 - mu) ** 2).mean(1, keepdim=True)
-    rstd = (var + EPS).rsqrt()
-    xhat = (pre64 - mu) * rstd
-    D = (tau * mag + (math.log2(N) + 4) * U * pre64.abs()).amax(1, keepdim=True)
-    g, b = gamma.double().abs(), beta.double().abs()
-    return rstd * g * (2 + xhat.abs()) * D + 4 * U * ((xhat * g).abs() + b)
-
-
 def ln_params(N, seed):
     return 1.0 + 0.1 * draw((N,), "mixed", seed), 0.1 * draw((N,), "mixed", seed + 1)
 
@@ -242,7 +226,7 @@ def test_gemm_ln_precision(cu, N, act):
         # SiLU: |silu'| <= 1.1, plus 4 u |out| for expf and the division
         slope = 1.1 if act else 1.0
         for name, o, tau in (("highest", o3, tau3(K)), ("high", o1, BAND[1])):
-            bound = slope * ln_bound(pre64, mag, gamma, beta, tau) + 4 * U * ref.abs()
+            bound = slope * ln_bound(pre64, mag, gamma, beta, tau, EPS) + 4 * U * ref.abs()
             out_margin[name] = max(out_margin[name], float(((o.double() - ref).abs() / bound).max()))
     assess(f"gemm_ln_N{N}_act{act}", K, errs, {"out/bound": out_margin["highest"], "out_high/bound": out_margin["high"]})
     assert out_margin["highest"] <= 1.0 and out_margin["high"] <= 1.0, out_margin
@@ -273,7 +257,7 @@ def test_gemm_ln_gru_precision(cu, N):
         c = torch.tanh(r * gc)
         dr, dc, du = (u * (1 - c * c) * gc * r * (1 - r)).abs(), u * (1 - c * c) * r, ((c - h_prev.double()) * u * (1 - u)).abs()
         for name, h, tau in (("highest", h3, tau3(K)), ("high", h1, BAND[1])):
-            br, bc, bu = torch.chunk(ln_bound(pre64, mag, gamma, beta, tau), 3, -1)
+            br, bc, bu = torch.chunk(ln_bound(pre64, mag, gamma, beta, tau, EPS), 3, -1)
             bound = dr * br + dc * bc + du * bu + 16 * U * (1 + h_prev.double().abs())
             h_margin[name] = max(h_margin[name], float(((h.double() - h64).abs() / bound).max()))
     assess(f"gemm_ln_gru_N{N}", K, errs, {"h/bound": h_margin["highest"], "h_high/bound": h_margin["high"]})

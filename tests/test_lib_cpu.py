@@ -29,6 +29,16 @@ WGRAD_TC = {               # NB, h, w, Cs, Cb -> b200rl_conv_wgrad_tc_supported
     "Cb7": (1, 32, 32, 48, 7, False), "P2e9": (2000000000, 1, 1, 48, 8, True),
     "P_above_2e9": (2000000001, 1, 1, 48, 8, False),
 }
+LN_ROUTE = {               # C, row stride (all three rows), base offset of (row 0, row 1, row 2, gamma) -> route
+    "vec_C32": (32, 32, (0, 0, 0, 0), 1), "vec_C48": (48, 48, (0, 0, 0, 0), 1), "vec_C640": (640, 640, (0, 0, 0, 0), 1),
+    "vec_C1536": (1536, 1536, (0, 0, 0, 0), 1), "vec_C256_ld260": (256, 260, (0, 0, 0, 0), 1),
+    "vec_C256_ld257": (256, 257, (0, 0, 0, 0), 0), "vec_C256_dX_misaligned": (256, 256, (0, 0, 1, 0), 0),
+    "vec_C256_gamma_misaligned": (256, 256, (0, 0, 0, 1), 0), "C100": (100, 100, (0, 0, 0, 0), 0),
+    "C1537": (1537, 1540, (0, 0, 0, 0), 0), "C2050_not_multiple_of_4": (2050, 2052, (0, 0, 0, 0), 0),
+    "wide_C1540": (1540, 1540, (0, 0, 0, 0), 2), "wide_C16384": (16384, 16384, (0, 0, 0, 0), 2),
+    "C16388": (16388, 16388, (0, 0, 0, 0), 0), "wide_C3072_ld3073": (3072, 3073, (0, 0, 0, 0), 0),
+    "wide_C3072_X_misaligned": (3072, 3072, (1, 0, 0, 0), 0), "C1": (1, 1, (0, 0, 0, 0), 0),
+}
 ADDR = 1 << 20             # synthetic 16-byte aligned device address: the queries compare pointer values only
 
 
@@ -141,6 +151,16 @@ def test_onehot_linear_ln_query_alignment(lib):
     assert not lib.b200rl_onehot_linear_ln_supported(ADDR, 2 * ADDR + 4, 3 * ADDR, 4 * ADDR, None, 128, 128, 0)
     assert not lib.b200rl_onehot_linear_ln_supported(ADDR, 2 * ADDR, 3 * ADDR, 4 * ADDR, 5 * ADDR + 8, 128, 128, 128)
     assert not lib.b200rl_onehot_linear_ln_supported(ADDR, 2 * ADDR, 3 * ADDR, 4 * ADDR, 5 * ADDR, 128, 128, 130)
+
+
+@pytest.mark.parametrize("case", list(LN_ROUTE))
+def test_ln_act_route_query(lib, case):
+    C, ld, (o0, o1, o2, og), route = LN_ROUTE[case]
+    assert lib.b200rl_ln_act_route(C, ld, ld, ld, ADDR + 4 * o0, 2 * ADDR + 4 * o1, 3 * ADDR + 4 * o2, 4 * ADDR + 4 * og,
+                                   5 * ADDR) == route
+    if o2 == 0:                # the forward passes no third row: ld2 = 0, p2 = NULL
+        assert lib.b200rl_ln_act_route(C, ld, ld, 0, ADDR + 4 * o0, 2 * ADDR + 4 * o1, None, 4 * ADDR + 4 * og,
+                                       5 * ADDR) == route
 
 
 @pytest.mark.parametrize("case", list(WGRAD_TC))
