@@ -106,10 +106,11 @@ def build_agent(
     """ops (extra, optional): the kernel binding; default `sheeprl_b200.lib.CudaOps` (tests on a GPU-less host pass the
     torch test double)."""
     cnn_keys, mlp_keys = list(cfg.algo.cnn_keys.encoder or []), list(cfg.algo.mlp_keys.encoder or [])
-    in_channels = sum(int(math.prod(obs_space[k].shape[:-2])) for k in cnn_keys) if cnn_keys else 3    # agent.py:984
+    cnn_dims = {k: int(math.prod(obs_space[k].shape[:-2])) for k in cnn_keys}       # agent.py:984, 1070
+    in_channels = sum(cnn_dims.values()) if cnn_keys else 3
     mlp_dims = {k: int(obs_space[k].shape[0]) for k in mlp_keys}          # agent.py:1002
     eng = DV3Engine(cfg, actions_dim, in_channels=in_channels, device=fabric.device, ops=ops if ops is not None else DEFAULT_OPS,
-                    is_continuous=is_continuous, mlp_dims=mlp_dims)
+                    is_continuous=is_continuous, mlp_dims=mlp_dims, cnn_dims=cnn_dims)
     seed, rank = int(cfg.get("seed", 0) or 0), int(getattr(fabric, "global_rank", 0) or 0)
     eng.rng_seed = (seed * 1000003 + rank) & 0x7FFFFFFF        # sampling noise follows cfg.seed; ranks draw different streams
     if int(getattr(fabric, "world_size", 1) or 1) > 1:
@@ -129,9 +130,10 @@ def build_agent(
     wm_scale = {"rssm.transition_model._model.3.weight": 1.0, "rssm.representation_model._model.3.weight": 1.0,
                 f"reward_model._model.{3 * nh}.weight": 0.0, f"continue_model._model.{3 * nh}.weight": 1.0} if haf else {}
     if haf:
-        wm_scale.update({f"observation_model.mlp_decoder.heads.{i}.weight": 1.0 for i in range(len(mlp_keys))})   # agent.py:1177-1178
+        # one head per decoded vector key (agent.py:1177-1178)
+        wm_scale.update({f"observation_model.mlp_decoder.heads.{i}.weight": 1.0 for i in range(len(eng.dec_vec_keys))})
     wm_init = initial_state(eng.wm, wm_scale, g)
-    if haf and cnn_keys:
+    if haf and eng.has_cnn_dec:
         # `uniform_init_weights` only touches nn.Linear / nn.LayerNorm (dreamer_v3/utils.py:170-186): applied to the
         # last ConvTranspose2d (agent.py:1180) it is a no-op, so that layer keeps its truncated-normal init.
         assert last_dec in wm_init

@@ -25,21 +25,39 @@ class PlayerDV3:
         """actor_group: the flat group of the policy that acts (default the trainer's task actor; Plan2Explore passes
         its exploration actor when `algo.player.actor_type == "exploration"`, p2e_dv3/agent.py:206-212)"""
         self.trainer = engine
-        self.num_envs = int(num_envs)
         self.actor_type = actor_type
         self.actions_dim = engine.actions_dim
         self.device = engine.device
         self.stochastic_size, self.discrete_size = engine.S, engine.D
         self.recurrent_state_size = engine.R
+        self._actor_group = actor_group or engine.actor
+        self._num_envs = None
+        self.num_envs = num_envs
+        self._counter = torch.zeros(1, dtype=torch.int32, device=self.device)
+        self.rng_seed = 0x5EED
+
+    @property
+    def num_envs(self) -> int:
+        return self._num_envs
+
+    @num_envs.setter
+    def num_envs(self, n) -> None:
+        """The acting engine and the state tensors are sized for `n` rows; a new `n` re-creates them over the same
+        parameter groups (the reference's `test()` sets `player.num_envs = 1`, then calls `init_states()`)."""
+        n = int(n)
+        if n == self._num_envs:
+            return
+        self._num_envs = n
+        engine = self.trainer
         cfg = copy.deepcopy(engine.cfg)
         cfg.algo.per_rank_sequence_length = 1
-        cfg.algo.per_rank_batch_size = self.num_envs
+        cfg.algo.per_rank_batch_size = n
         cfg.algo.horizon = 1
         self.eng = DV3Engine(cfg, engine.actions_dim, in_channels=engine.Cin, device=engine.device, ops=engine.ops,
                              is_continuous=engine.is_continuous,
-                             groups=(engine.wm, actor_group or engine.actor, engine.critic, engine.target),
-                             mlp_dims=dict(zip(engine.vec_keys, engine.vec_dims)))
-        e, E = self.eng, self.num_envs
+                             groups=(engine.wm, self._actor_group, engine.critic, engine.target),
+                             mlp_dims=dict(zip(engine.vec_keys, engine.vec_dims)), cnn_dims=engine.cnn_dims)
+        e, E = self.eng, n
         f = lambda *s: torch.zeros(*s, dtype=torch.float32, device=self.device)  # noqa: E731
         # persistent acting state (reference attribute names; leading dim 1 as in the reference)
         self.actions = f(1, E, e.A)
@@ -47,8 +65,6 @@ class PlayerDV3:
         self.stochastic_state = f(1, E, e.Z)
         self._h_next = f(E, e.R)
         self._noise_z, self._noise_a = f(E, e.Z), f(E, e.A)
-        self._counter = torch.zeros(1, dtype=torch.int32, device=self.device)
-        self.rng_seed = 0x5EED
 
     # ------------------------------------------------------------------ reference surface
     class _ActorInfo:
@@ -81,9 +97,9 @@ class PlayerDV3:
                     noise: Optional[Dict[str, torch.Tensor]] = None) -> Sequence[torch.Tensor]:
         """obs[key]: `[1, num_envs, C, H, W]` — float32 already normalised as the reference's `prepare_obs` passes it
         (dreamer_v3/utils.py:80-91), or raw uint8 (normalised by the kernel: 4x less host->device traffic).
-        `noise` (extra, optional): {"z": Exp(1) [E, S*D], "a": Exp(1) / N(0,1) [E, A]} for parity tests."""
-        if mask is not None:
-            raise NotImplementedError("action masks (MineDojo actor) are not built")
+        `noise` (extra, optional): {"z": Exp(1) [E, S*D], "a": Exp(1) / N(0,1) [E, A]} for parity tests.
+        `mask` is ignored, as the reference's `Actor.forward` ignores it (the reference's `test()` passes the observation's
+        `mask*` keys, an empty dict for environments without them)."""
         e, ops, E = self.eng, self.eng.ops, self.num_envs
         Z = e.Z
         if e.has_cnn:

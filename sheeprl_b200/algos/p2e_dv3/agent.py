@@ -40,15 +40,17 @@ def build_agent(
     ops=None,
 ):
     cnn_keys, mlp_keys = list(cfg.algo.cnn_keys.encoder or []), list(cfg.algo.mlp_keys.encoder or [])
-    in_channels = sum(int(math.prod(obs_space[k].shape[:-2])) for k in cnn_keys) if cnn_keys else 3    # agent.py:984
+    cnn_dims = {k: int(math.prod(obs_space[k].shape[:-2])) for k in cnn_keys}
+    in_channels = sum(cnn_dims.values()) if cnn_keys else 3    # agent.py:984
     eng = P2EDV3Engine(cfg, actions_dim, in_channels=in_channels, device=fabric.device, ops=ops, is_continuous=is_continuous,
-                       mlp_dims={k: int(obs_space[k].shape[0]) for k in mlp_keys})
+                       mlp_dims={k: int(obs_space[k].shape[0]) for k in mlp_keys}, cnn_dims=cnn_dims)
     seed = int(cfg.get("seed", 0) or 0)
     g = torch.Generator().manual_seed(seed)
     nh, haf = cfg.algo.mlp_layers, bool(cfg.algo.hafner_initialization)
     wm_scale = {"rssm.transition_model._model.3.weight": 1.0, "rssm.representation_model._model.3.weight": 1.0,
                 f"reward_model._model.{3 * nh}.weight": 0.0, f"continue_model._model.{3 * nh}.weight": 1.0,
-                **{f"observation_model.mlp_decoder.heads.{i}.weight": 1.0 for i in range(len(mlp_keys))}} if haf else {}
+                **{f"observation_model.mlp_decoder.heads.{i}.weight": 1.0
+                   for i in range(len(cfg.algo.mlp_keys.decoder or []))}} if haf else {}
     n_heads = 1 if is_continuous else len(actions_dim)
     ac_scale = {f"mlp_heads.{i}.weight": 1.0 for i in range(n_heads)} if haf else {}
     cr_scale = {f"_model.{3 * nh}.weight": 0.0} if haf else {}

@@ -50,18 +50,19 @@ class P2EDV3Engine(DV3Engine):
     METRIC_NAMES_P2E = ("Loss/ensemble_loss", "Loss/policy_loss_exploration")
 
     def __init__(self, cfg, actions_dim: Sequence[int], in_channels: int = 3, device="cuda", ops=None,
-                 is_continuous: bool = False, mlp_dims=None):
+                 is_continuous: bool = False, mlp_dims=None, cnn_dims=None):
         if cfg.algo.world_model.decoupled_rssm:
             raise NotImplementedError(
                 "Plan2Explore cannot run with decoupled_rssm: the reference's exploration train() calls the five-argument "
                 "RSSM.dynamic (p2e_dv3_exploration.py:136), which DecoupledRSSM does not have")
-        super().__init__(cfg, actions_dim, in_channels, device, ops, is_continuous=is_continuous, mlp_dims=mlp_dims)
+        super().__init__(cfg, actions_dim, in_channels, device, ops, is_continuous=is_continuous, mlp_dims=mlp_dims,
+                         cnn_dims=cnn_dims)
         a = cfg.algo
         N, H, L, A, Z = self.N, self.H, self.L, self.A, self.Z
         M1, M0 = (H + 1) * N, H * N
         b = self._buf
         _, ac_s, cr_s, _ = dv3_param_shapes(cfg, self.actions_dim, in_channels, self.is_continuous,
-                                            dict(zip(self.vec_keys, self.vec_dims)))
+                                            dict(zip(self.vec_keys, self.vec_dims)), self.cnn_dims)
         # ---- exploration actor and critics
         self.actor_expl = FlatGroup(ac_s, device)
         self.actor_expl_mlp = _MLP(self, self.actor_expl, "model._model.", L, self.du, self.nh, None, M1, self.eps,

@@ -32,11 +32,42 @@ ACT_NONE, ACT_SILU = 0, 1
 TWOHOT_LOW, TWOHOT_HIGH = -20.0, 20.0
 
 
+def decoder_channels(cfg, in_channels: int, cnn_dims: Optional[Mapping[str, int]] = None) -> int:
+    """Channels of the CNN decoder's output: the sum over cfg.algo.cnn_keys.decoder (CNNDecoder, agent.py:1067-1081).
+    cnn_dims: {image key: channels}; not needed when the decoder's keys are the encoder's, in the same order."""
+    a = cfg.algo
+    dec = list(a.cnn_keys.decoder or [])
+    if dec == list(a.cnn_keys.encoder or []):
+        return in_channels
+    missing = [k for k in dec if k not in (cnn_dims or {})]
+    if missing:
+        raise ValueError(f"the channel count of the decoded image key(s) {missing} is not known (pass cnn_dims)")
+    return sum(int(cnn_dims[k]) for k in dec)
+
+
+def check_decoder_keys(cfg) -> None:
+    """The decoders reconstruct a subset of the encoded keys (the reference's main, dreamer_v3.py:413-427; its train()
+    fails with a KeyError on a decoder key that is not encoded)"""
+    a = cfg.algo
+    for kind in ("cnn_keys", "mlp_keys"):
+        enc, dec = list(a[kind].encoder or []), list(a[kind].decoder or [])
+        for k in dec:
+            if k not in enc:
+                raise ValueError(f"{kind}.decoder: key '{k}' is not in {kind}.encoder {enc}: the decoder can only "
+                                 f"reconstruct encoded keys")
+        if len(set(dec)) != len(dec):
+            raise ValueError(f"{kind}.decoder names a key twice: {dec}")
+    if not a.cnn_keys.decoder and not a.mlp_keys.decoder:
+        raise ValueError("There must be at least one decoder: cnn_keys.decoder and mlp_keys.decoder are both empty")
+
+
 def dv3_param_shapes(cfg, actions_dim: Sequence[int], in_channels: int, is_continuous: bool = False,
-                     mlp_dims: Optional[Mapping[str, int]] = None):
+                     mlp_dims: Optional[Mapping[str, int]] = None, cnn_dims: Optional[Mapping[str, int]] = None):
     """Shapes keyed by the reference's state-dict names (SURVEY.md §8b; built in agent.py:935-1180).
     mlp_dims: {vector observation key: dimension} for the keys of cfg.algo.mlp_keys (MLPEncoder / MLPDecoder,
-    agent.py:100-152, 229-278); the CNN encoder / decoder exist only when cfg.algo.cnn_keys.encoder is not empty."""
+    agent.py:100-152, 229-278); the CNN encoder exists only when cfg.algo.cnn_keys.encoder is not empty, the CNN / MLP
+    decoder only when cfg.algo.cnn_keys.decoder / mlp_keys.decoder is not empty.  cnn_dims: {image key: channels}, for
+    a CNN decoder over other keys than the encoder's (`decoder_channels`)."""
     a, w = cfg.algo, cfg.algo.world_model
     S, D = w.stochastic_size, w.discrete_size
     Z, R = S * D, w.recurrent_model.recurrent_state_size
@@ -81,11 +112,13 @@ def dv3_param_shapes(cfg, actions_dim: Sequence[int], in_channels: int, is_conti
     mlp(wm, "rssm.representation_model._model.", (0 if w.decoupled_rssm else R) + E + Ev,
         w.representation_model.hidden_size, 1, Z)
     mlp(wm, "rssm.transition_model._model.", R, w.transition_model.hidden_size, 1, Z)
-    if has_cnn:
+    has_cnn_dec = len(a.cnn_keys.decoder or []) > 0
+    if has_cnn_dec:
         wm["observation_model.cnn_decoder.model.0.weight"] = (E, L)
         wm["observation_model.cnn_decoder.model.0.bias"] = (E,)
-    dch = [chans[-1]] + [mult * 2 ** i for i in reversed(range(stages - 1))] + [in_channels]
-    for i in range(stages if has_cnn else 0):
+    dch = [chans[-1]] + [mult * 2 ** i for i in reversed(range(stages - 1))] + [
+        decoder_channels(cfg, in_channels, cnn_dims) if has_cnn_dec else in_channels]
+    for i in range(stages if has_cnn_dec else 0):
         p = f"observation_model.cnn_decoder.model.2._model.{3 * i}"
         wm[p + ".weight"] = (dch[i], dch[i + 1], 4, 4)
         if i == stages - 1:
@@ -228,10 +261,13 @@ class _MLP:
 
 class DV3Engine:
     def __init__(self, cfg, actions_dim: Sequence[int], in_channels: int = 3, device="cuda", ops=None,
-                 is_continuous: bool = False, groups=None, mlp_dims: Optional[Mapping[str, int]] = None):
+                 is_continuous: bool = False, groups=None, mlp_dims: Optional[Mapping[str, int]] = None,
+                 cnn_dims: Optional[Mapping[str, int]] = None):
         """groups: optional (wm, actor, critic, target) FlatGroups to adopt instead of allocating new ones — the acting
         engine of PlayerDV3 shares the trainer's parameters this way (the reference ties `.data`, agent.py:1229-1235).
-        mlp_dims: {key: dimension} of the vector observations named in cfg.algo.mlp_keys (default: cfg.env.mlp_dims)."""
+        mlp_dims: {key: dimension} of the vector observations named in cfg.algo.mlp_keys (default: cfg.env.mlp_dims).
+        cnn_dims: {key: channels} of the image keys; needed only when cnn_keys.decoder differs from cnn_keys.encoder
+        (default: cfg.env.cnn_channels)."""
         a, w = cfg.algo, cfg.algo.world_model
         self.is_continuous = bool(is_continuous)
         if self.is_continuous and str(cfg.distribution.get("type", "auto")).lower() not in ("auto", "scaled_normal"):
@@ -240,16 +276,28 @@ class DV3Engine:
                 "with tanh_normal (entropy fallback shape, dreamer_v3.py:294-297) and normal (negative scale)")
         self.decoupled = bool(w.decoupled_rssm)           # DecoupledRSSM (agent.py:501-593): z_t does not depend on h_t
         _check_supported_modules(cfg)
-        if list(a.cnn_keys.encoder) != list(a.cnn_keys.decoder) or list(a.mlp_keys.encoder) != list(a.mlp_keys.decoder):
-            raise NotImplementedError("the decoder must reconstruct exactly the encoder's keys")
         if not a.cnn_keys.encoder and not a.mlp_keys.encoder:
             raise ValueError("There must be at least one encoder, both cnn and mlp encoders are None")     # models.py:420-421
+        check_decoder_keys(cfg)
+        actor_cls = str(a.actor.get("cls", "Actor"))
+        if actor_cls.endswith("MinedojoActor"):
+            raise NotImplementedError(f"algo.actor.cls = {actor_cls}: the action masks of the MineDojo actor are not built")
         self.cnn_keys = list(a.cnn_keys.encoder)          # several image keys: concatenated on the channel axis (agent.py:96)
         self.has_cnn = len(self.cnn_keys) > 0
         self.vec_keys = list(a.mlp_keys.encoder)
         vd = dict(mlp_dims if mlp_dims is not None else (cfg.env.get("mlp_dims", None) or {}))
         self.vec_dims = [int(vd[k]) for k in self.vec_keys]
         self.Dv = sum(self.vec_dims)
+        # decoders: a subset of the encoded keys, in their own order (heads and the CNN output split follow it)
+        self.dec_cnn_keys = list(a.cnn_keys.decoder or [])
+        self.has_cnn_dec = len(self.dec_cnn_keys) > 0
+        self.cnn_dec_same = self.dec_cnn_keys == self.cnn_keys         # target = the encoder's input x0
+        self.dec_vec_keys = list(a.mlp_keys.decoder or [])
+        self.dec_vec_dims = [int(vd[k]) for k in self.dec_vec_keys]
+        self.has_vec_dec = len(self.dec_vec_keys) > 0
+        self.vec_dec_same = self.dec_vec_keys == self.vec_keys          # target = the encoder's input vx
+        self.Dvd = sum(self.dec_vec_dims)
+        self.cnn_dims = dict(cnn_dims if cnn_dims is not None else (cfg.env.get("cnn_channels", None) or {}))
         if ops is None:
             from sheeprl_b200.lib import CudaOps  # raises loudly if the extension / a GPU is missing
 
@@ -276,8 +324,9 @@ class DV3Engine:
         self.img = cfg.env.screen_size
         self.key = a.cnn_keys.encoder[0] if self.has_cnn else None
         self.bins_r, self.bins_c = w.reward_model.bins, a.critic.bins
+        self.Cdec = decoder_channels(cfg, in_channels, self.cnn_dims) if self.has_cnn_dec else 0
         wm_s, ac_s, cr_s, meta = dv3_param_shapes(cfg, self.actions_dim, in_channels, self.is_continuous,
-                                                  dict(zip(self.vec_keys, self.vec_dims)))
+                                                  dict(zip(self.vec_keys, self.vec_dims)), self.cnn_dims)
         self.Ev = meta["Ev"]                                      # width of the vector-encoder features (0: none)
         self.AW = 2 * self.A if self.is_continuous else self.A          # width of the actor head output
         self.chans, self.dch, self.E, self.stages = meta["chans"], meta["dch"], meta["E"], meta["stages"]
@@ -324,17 +373,21 @@ class DV3Engine:
             self.enc_a.append(b(f"enc_a{i}", N, s, s, self.chans[i + 1]))
         self.emb = b("emb", N, E) if self.has_cnn else None
         self.pe = b("pe", N, self.Dr)
+        we, wo = self.cfg.algo.world_model.encoder, self.cfg.algo.world_model.observation_model
         if self.vec_keys:
-            # vector observations: vx = symlog(concat(obs_k)) is the MLP encoder's input AND the MLP decoder's target
-            we, wo = self.cfg.algo.world_model.encoder, self.cfg.algo.world_model.observation_model
+            # vector observations: vx = symlog(concat(obs_k)) is the MLP encoder's input, and the MLP decoder's target
+            # when that decodes the same keys in the same order
             self.vx = b("vx", N, self.Dv)
             self.venc = _MLP(self, self.wm, "encoder.mlp_encoder.model._model.", self.Dv, we.dense_units, we.mlp_layers, None,
                              N, float(we.mlp_layer_norm.kw.eps), "venc", True)
             self.d_emb_vec = b("d_emb_vec", N, self.Ev)
+        if self.has_vec_dec:
             self.vdec = _MLP(self, self.wm, "observation_model.mlp_decoder.model._model.", L, wo.dense_units, wo.mlp_layers,
                              None, N, float(wo.mlp_layer_norm.kw.eps), "vdec", True)
-            self.vrecon, self.vec_rows = b("vrecon", N, self.Dv), b("vec_rows", N)
+            self.vrecon, self.vec_rows = b("vrecon", N, self.Dvd), b("vec_rows", N)
             self.d_vdec_hidden = b("d_vdec_hidden", N, wo.dense_units)
+            # symlog(concat(obs_k)) over the decoder's keys in decoder order
+            self.vtgt = self.vx if self.vec_dec_same else b("vtgt", N, self.Dvd)
         self.traj = b("traj", H + 1, N, L)
         self.latent = self.traj[0]
         # scan saves
@@ -366,6 +419,7 @@ class DV3Engine:
         self.dec_y, self.dec_a, self.d_dec_a, self.d_enc_a = [], [], [], []
         if self.has_cnn:
             self.d_emb = b("d_emb", N, E)
+        if self.has_cnn_dec:
             # decoder
             self.dec_lin = b("dec_lin", N, E)
             C0 = self.dch[0]
@@ -375,10 +429,13 @@ class DV3Engine:
                 s *= 2
                 self.dec_y.append(b(f"dec_y{i}", N, s, s, self.dch[i + 1]))
                 self.dec_a.append(b(f"dec_a{i}", N, s, s, self.dch[i + 1]))
-            self.recon = b("recon", N, img, img, self.Cin)
+            self.recon = b("recon", N, img, img, self.Cdec)
             self.d_dec_in = b("d_dec_in", N, 4, 4, C0)
             self.d_dec_lin = b("d_dec_lin", N, E)
             self.d_dec_a = [b(f"d_dec_a{i}", *self.dec_a[i].shape) for i in range(self.stages - 1)]
+            # the decoder's target: the encoder's input, else the normalised pixels of the decoder's keys
+            self.x_dec = self.x0 if self.cnn_dec_same else b("x_dec", N, img, img, self.Cdec)
+        if self.has_cnn:
             self.d_enc_a = [b(f"d_enc_a{i}", *self.enc_a[i].shape) for i in range(self.stages)]
         # losses
         self.obs_rows, self.rew_rows, self.cont_rows = b("obs_rows", N), b("rew_rows", N), b("cont_rows", N)
@@ -560,6 +617,13 @@ class DV3Engine:
         for k, d in zip(self.vec_keys, self.vec_dims):       # symlog squashing (MLPEncoder.forward, agent.py:150)
             ops.symlog(data[k].reshape(N, d), self.vx[:, off:off + d])
             off += d
+        if self.has_cnn_dec and not self.cnn_dec_same:
+            ops.obs_prep(self.image_batch(data, N, self.dec_cnn_keys), self.x_dec)
+        if self.has_vec_dec and not self.vec_dec_same:
+            off = 0
+            for k, d in zip(self.dec_vec_keys, self.dec_vec_dims):
+                ops.symlog(data[k].reshape(N, d), self.vtgt[:, off:off + d])
+                off += d
         data["is_first"][0].fill_(1.0)                      # same in-place mutation as the reference (:100)
         first = data["is_first"].reshape(N)
         ops.zero(self.shift_actions[:B])
@@ -578,15 +642,16 @@ class DV3Engine:
 
         # ---- losses + seed gradients (loss.py:9-88); mean over T*B
         inv = 1.0 / N
-        if self.has_cnn:
-            P = self.img * self.img * self.Cin
-            ops.mse_loss_grad(self.recon.view(N, P), self.x0.view(N, P), inv, self.obs_rows, self.recon.view(N, P))
-        if self.vec_keys:
+        if self.has_cnn_dec:
+            # MSEDistribution per decoded key (loss.py:61): the per-key sums add up to one sum over the channels
+            P = self.img * self.img * self.Cdec
+            ops.mse_loss_grad(self.recon.view(N, P), self.x_dec.view(N, P), inv, self.obs_rows, self.recon.view(N, P))
+        if self.has_vec_dec:
             # SymlogDistribution (utils/distribution.py:177-192): squared error against symlog(obs), summed over keys and
             # dims (its `tol` = 1e-8 cut on the squared distance is not reproduced: |effect| < 1e-8 per element)
-            rows = self.vec_rows if self.has_cnn else self.obs_rows
-            ops.mse_loss_grad(self.vrecon, self.vx, inv, rows, self.vrecon)
-            if self.has_cnn:
+            rows = self.vec_rows if self.has_cnn_dec else self.obs_rows
+            ops.mse_loss_grad(self.vrecon, self.vtgt, inv, rows, self.vrecon)
+            if self.has_cnn_dec:
                 ops.axpy(self.vec_rows, self.obs_rows)
         ops.twohot_loss_grad(rew_logits, rewards, None, inv, TWOHOT_LOW, TWOHOT_HIGH, self.rew_rows, self.d_rew_logits)
         ops.bce_loss_grad(cont_logit, self.true_cont, float(w.continue_scale_factor), inv, self.cont_rows,
@@ -640,16 +705,19 @@ class DV3Engine:
         p = "observation_model.cnn_decoder.model.2._model."
         return f"{p}{3 * i}.weight", f"{p}{3 * i + 1}.weight", f"{p}{3 * i + 1}.bias"
 
-    def image_batch(self, obs: Dict[str, torch.Tensor], rows: int) -> torch.Tensor:
-        """[rows, Cin, H, W] pixels (uint8 or float) of the image key(s); more than one key is concatenated on the channel
-        axis, as CNNEncoder.forward does on every call (agent.py:96) — a device copy, no arithmetic"""
-        imgs = [obs[k].reshape(rows, -1, self.img, self.img) for k in self.cnn_keys]
+    def image_batch(self, obs: Dict[str, torch.Tensor], rows: int, keys: Optional[Sequence[str]] = None) -> torch.Tensor:
+        """[rows, C, H, W] pixels (uint8 or float) of the image key(s) (default: the encoder's); more than one key is
+        concatenated on the channel axis, as CNNEncoder.forward does on every call (agent.py:96) — a device copy, no
+        arithmetic.  `keys`: the CNN decoder's keys, whose concatenation is its target."""
+        keys = self.cnn_keys if keys is None else keys
+        C = self.Cin if keys is self.cnn_keys else self.Cdec
+        imgs = [obs[k].reshape(rows, -1, self.img, self.img) for k in keys]
         if len(imgs) == 1:
             return imgs[0]
         if any(t.dtype != imgs[0].dtype for t in imgs):
             imgs = [t.float() for t in imgs]
         out = torch.cat(imgs, 1)
-        assert out.shape[1] == self.Cin, f"image keys carry {out.shape[1]} channels, the encoder was built for {self.Cin}"
+        assert out.shape[1] == C, f"image keys {keys} carry {out.shape[1]} channels, the network was built for {C}"
         return out
 
     def _project_embedding(self, out: torch.Tensor):
@@ -702,18 +770,18 @@ class DV3Engine:
     def _vec_heads(self):
         """[(head weight name, column offset, width)] of the MLP decoder's per-key output layers"""
         out, off = [], 0
-        for i, d in enumerate(self.vec_dims):
+        for i, d in enumerate(self.dec_vec_dims):
             out.append((f"observation_model.mlp_decoder.heads.{i}", off, d))
             off += d
         return out
 
     def _decoder_forward(self):
         ops = self.ops
-        if self.vec_keys:
+        if self.has_vec_dec:
             hid = self.vdec.forward(self.latent)
             for name, off, d in self._vec_heads():
                 ops.gemm(hid, self._w(name + ".weight"), self.vrecon[:, off:off + d], False, True, bias=self._w(name + ".bias"))
-        if not self.has_cnn:
+        if not self.has_cnn_dec:
             return
         p = "observation_model.cnn_decoder.model."
         ops.gemm(self.latent, self._w(p + "0.weight"), self.dec_lin, False, True, bias=self._w(p + "0.bias"))
@@ -731,11 +799,12 @@ class DV3Engine:
         ops.conv_up(cur, self._w(wn), self.recon, bias=self._w(wn.replace(".weight", ".bias")))
 
     def _decoder_backward(self):
-        """self.recon / self.vrecon hold d(loss)/d(reconstruction) (written in place by mse_loss_grad). Writes d_latent."""
+        """self.recon / self.vrecon hold d(loss)/d(reconstruction) (written in place by mse_loss_grad). Writes d_latent:
+        the first decoder writes it, the second accumulates."""
         ops = self.ops
-        if self.has_cnn:
+        if self.has_cnn_dec:
             self._cnn_decoder_backward()
-        if self.vec_keys:
+        if self.has_vec_dec:
             hid = self.vdec.act[-1]
             ops.zero(self.d_vdec_hidden)
             for name, off, d in self._vec_heads():
@@ -743,14 +812,14 @@ class DV3Engine:
                 ops.gemm(dv, hid, self._gw(name + ".weight"), True, False)
                 ops.col_sum(dv, self._gw(name + ".bias"))
                 ops.gemm(dv, self._w(name + ".weight"), self.d_vdec_hidden, False, False, accumulate=True)
-            self.vdec.backward(self.latent, self.d_vdec_hidden, self.d_latent, self.has_cnn)
+            self.vdec.backward(self.latent, self.d_vdec_hidden, self.d_latent, self.has_cnn_dec)
 
     def _cnn_decoder_backward(self):
         ops = self.ops
         st = self.stages
         wn = self._dec_names(st - 1)[0]
         d_big = self.recon
-        ops.col_sum(d_big.view(-1, self.Cin), self._gw(wn.replace(".weight", ".bias")))
+        ops.col_sum(d_big.view(-1, self.Cdec), self._gw(wn.replace(".weight", ".bias")))
         for i in reversed(range(st)):
             wn, gn, bn = self._dec_names(i)
             inp = self.dec_in if i == 0 else self.dec_a[i - 1]
