@@ -178,6 +178,8 @@ int b200rl_head_sample(const float* X, const float* W, const float* bias, const 
 int b200rl_cat_sample_bwd(const float* raw, const float* dz, const float* dmix, float* draw, long long M, int groups,
                           int classes, long long ldr, long long lddz, long long lddm, long long lddr, float unimix,
                           cudaStream_t stream);
+/* KL(post || prior) summed over the groups with free nats (loss.py), its rows and the gradients w.r.t. both mixes;
+ * held to a float64 reference with first-order error bounds (tests/test_gpu_loss_precision.py). */
 int b200rl_kl_loss_grad(const float* post_mix, const float* prior_mix, float* d_post, float* d_prior, float* rows,
                         long long M, int groups, int classes, long long ldp, long long ldq, long long lddp,
                         long long lddq, float kl_dyn, float kl_rep, float free_nats, float regularizer, float scale,
@@ -267,7 +269,8 @@ int b200rl_gru_scan_check(const b200rl_gru_scan_args* args, int backward);
 /* ---- losses (value + seed gradient) -----------------------------------------------------------------
  * distribution.py:212-276 (MSE, two-hot on symlog), Bernoulli continue head loss.py:77, lambda returns
  * dreamer_v3/utils.py:66-77 + dreamer_v3.py:244-260, Moments dreamer_v3/utils.py:40-63, discrete policy
- * loss dreamer_v3.py:272-297. */
+ * loss dreamer_v3.py:272-297.  Each is held to a float64 reference with per-element first-order error bounds, and
+ * moments_update to torch.quantile's order statistics, NaN included (tests/test_gpu_loss_precision.py). */
 int b200rl_mse_loss_grad(const float* pred, const float* target, float* loss_row, float* grad, long long M, int P,
                          float scale, cudaStream_t stream);
 int b200rl_twohot_loss_grad(const float* logits, const float* x, const float* weight, float* loss_row, float* dlogits,
@@ -468,7 +471,8 @@ int b200rl_onehot_linear_ln(const float* z, const float* act, const float* WT, c
 
 /* ---- Dreamer-V3 continuous actions (policy gradient through the imagined rollout) -------------------------
  * Actor.forward `scaled_normal` branch agent.py:803-825: head = [mean | std_raw] (M x 2A), eps ~ N(0,1);
- * action (row stride lda) = clip-rescaled tanh(mean) + std*eps, ent[M] = Independent(Normal).entropy(). */
+ * action (row stride lda) = clip-rescaled tanh(mean) + std*eps, ent[M] = Independent(Normal).entropy().  The four
+ * entry points below are held to a float64 reference with first-order error bounds (tests/test_gpu_loss_precision.py). */
 int b200rl_cont_action_fwd(const float* head, const float* eps, float* action, long long lda, float* ent, long long M,
                            int A, float min_std, float max_std, float init_std, float clip, cudaStream_t stream);
 /* its backward: d_action (row stride ldd) and the entropy bonus d_ent[m] = ent_scale * discount[m] -> dhead */

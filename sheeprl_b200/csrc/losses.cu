@@ -177,14 +177,17 @@ __device__ float select_kth(const float* __restrict__ x, long long n, long long 
   return key_float(prefix);
 }
 
+// torch.quantile 'linear' of NaN-free x: the fp32 rank q (n - 1), the order statistics at its floor and ceil, ATen's
+// lerp.  At an integral rank both are the same element, so the result is that element (an infinite one gives NaN, as
+// ATen's lerp(a, a, 0) does) and never a zero weight times the next order statistic.
 __device__ float quantile_linear(const float* x, long long n, float q, unsigned int* hist, unsigned int* bcast) {
   const float rank = q * (float)(n - 1);
   const float lo = floorf(rank);
   const long long ilo = (long long)lo;
-  const long long ihi = min(ilo + 1, n - 1);
+  const long long ihi = (long long)ceilf(rank);
   const float w = rank - lo;
   const float a = select_kth(x, n, ilo, hist, bcast);
-  const float b = select_kth(x, n, ihi, hist, bcast);
+  const float b = (ihi == ilo) ? a : select_kth(x, n, ihi, hist, bcast);
   return (w < 0.5f) ? (a + w * (b - a)) : (b - (b - a) * (1.f - w));  // ATen lerp
 }
 
@@ -193,15 +196,20 @@ moments_update_kernel(const float* __restrict__ x, long long n, float* __restric
                       float decay, float one_minus_decay, float inv_max, float p_low, float p_high) {
   __shared__ unsigned int hist[256];
   __shared__ unsigned int bcast[2];
-  const float lo = quantile_linear(x, n, p_low, hist, bcast);
-  const float hi = quantile_linear(x, n, p_high, hist, bcast);
+  int nan_seen = 0;
+  for (long long i = threadIdx.x; i < n; i += blockDim.x) nan_seen |= isnan(x[i]) ? 1 : 0;
+  // torch.quantile returns NaN for both quantiles when x holds a NaN
+  const bool any_nan = __syncthreads_or(nan_seen) != 0;
+  const float lo = any_nan ? NAN : quantile_linear(x, n, p_low, hist, bcast);
+  const float hi = any_nan ? NAN : quantile_linear(x, n, p_high, hist, bcast);
   if (threadIdx.x == 0) {
     const float l = decay * state[0] + one_minus_decay * lo;
     const float h = decay * state[1] + one_minus_decay * hi;
     state[0] = l;
     state[1] = h;
     out[0] = l;
-    out[1] = fmaxf(inv_max, h - l);
+    const float d = h - l;
+    out[1] = isnan(d) ? d : fmaxf(inv_max, d);  // torch.max propagates NaN; fmaxf would drop it
   }
 }
 
