@@ -159,7 +159,9 @@ __device__ __forceinline__ void row_head_grad(const float* hd, const float* act,
 
 // One CTA: B is a minibatch (<= a few thousand rows).  MASKED (ppo_recurrent.py:77-101): only rows with
 // mask != 0 count; the means are over their number n, advantages are normalised over them when n > 1, and the other
-// rows get zero gradients.
+// rows get zero gradients.  With no kept row (n = 0) the losses and every gradient are 0, where torch's mean over no
+// rows would be NaN: the recurrent engine never builds such a minibatch (it refuses an empty sequence), and a zero
+// update keeps a stray one from poisoning the parameters.
 template <bool MASKED>
 __global__ void __launch_bounds__(256) ppo_loss_kernel(const PpoLossArgs a) {
   __shared__ float red[32];
