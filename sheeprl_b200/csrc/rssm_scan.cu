@@ -22,12 +22,13 @@
 //   * No grid barriers.  Every cross-CTA hand-off is a flag-carrying data exchange ("LL": each 8-byte element is
 //     {fp32 value, 32-bit step tag}, written with one 64-bit store and polled with 64-bit loads straight from L2):
 //     the consumer spins on the very data it needs, so a hand-off costs one L2 store + one L2 load latency instead of
-//     release-fence + atomic counter + acquire + a dependent load.  Five hand-offs per forward step (z indices, x rows,
-//     LayerNorm partial statistics, h rows, rp rows), four per backward step.
+//     release-fence + atomic counter + acquire + a dependent load.  Four hand-offs per forward step (z indices, x rows,
+//     GRU LayerNorm partial statistics, h rows; then rp rows to the sampling units), four per backward step.
 //   * Work that does not depend on the newest hand-off is issued before waiting for it (the h-part of the GRU product
 //     runs while the x rows are still being built; input prefetches at step start).
-//   * z_{t-1} is one-hot per group, so z W_in^T is a gather of S weights per output from the CTA's W_in slice; the x
-//     LayerNorm runs on partial statistics exchanged with the values (like the GRU's), no CTA is a serial row owner.
+//   * z_{t-1} is one-hot per group, so z W_in^T is a gather of S weights per output from the CTA's W_in slice.  Every
+//     CTA receives all x rows anyway (the x-part of the GRU product needs them), so each computes the x LayerNorm
+//     statistics itself, with the same code and summation order: bit-identical on every CTA, no CTA is a row owner.
 //   * Products: the batch is one MMA tile high, so a warp takes an (8-column tile) x (K slice) item of m16n8k8 TF32 MMAs
 //     with the 3xTF32 split (fp32-accurate); K-slice partials are summed in a fixed order (bit-reproducible).
 #include "b200rl.h"
@@ -73,7 +74,7 @@ struct Workspace {
 };
 
 struct LLGeo {           // offsets (in u64 elements) inside the LL region; every buffer is double-buffered by step parity
-  size_t z, x, sx, s, h, r, a, b, c, d, sb, sc, sd, total;
+  size_t z, x, s, h, r, a, b, c, d, sb, sc, sd, total;
 };
 
 __host__ __device__ inline LLGeo make_ll(int S, int Dx, int R, int Dr, int Z) {
@@ -81,7 +82,6 @@ __host__ __device__ inline LLGeo make_ll(int S, int Dx, int R, int Dr, int Z) {
   size_t o = 0;
   g.z = o; o += 2 * (size_t)MAXB * S;            // forward: sampled class indices
   g.x = o; o += 2 * (size_t)MAXB * Dx;           //          x_pre rows
-  g.sx = o; o += 2 * (size_t)MAXB * SCAN_G * 2;  //          partial statistics of the x LayerNorm
   g.s = o; o += 2 * (size_t)MAXB * SCAN_G * 2;   //          partial statistics of the GRU LayerNorm
   g.h = o; o += 2 * (size_t)MAXB * R;            //          h rows
   g.r = o; o += 2 * (size_t)MAXB * Dr;           //          rp_pre rows
@@ -167,39 +167,77 @@ __device__ __forceinline__ float ll_wait(const u64* p, unsigned tag, Spin& sp) {
 // Receives rows x n values (n even; LL rows of stride ss elements, 16-byte aligned) into shared memory rows of stride ds.
 // Thread (row group, column pair): LL_UNROLL 16-byte loads in flight before the first tag is checked (one L2 round trip
 // per batch; 8 in the forward kernel, 4 in the register-tighter backward kernel where 8 spilled and measured slower).
-// (not inlined, like the product routines below: their hot loops then own the register file instead of sharing it with
-// every value the step loop keeps live — inlined, ptxas spilled inside the FFMA2 loops and the products ran 5x slower)
+// With `sums` (the backward's LayerNorm hand-offs: the producers send their per-CTA row sums (sum dxh, sum dxh*xh) right
+// after the rows), warp w also polls the SCAN_G partials of row sr0 + w (< sr0 + rows) in the same wave: they are loaded
+// before the rows, every retry re-polls the stale rows and partials together, and the partials are then summed in a
+// fixed order, scaled by `inv` into out1 / out2 [sr0 + w].  `sums` points at the row-sum block of the step's parity.
+// (inlined, like every helper of the step loops: as calls, ptxas saved and restored the step's live values around each
+// one, and with ~225 KB of shared memory per SM those spills miss L1.  Inlined, the S model's forward and backward took
+// 1.66 / 1.65 ms per launch on an H100 instead of 1.72 / 2.07 ms.)
 template <int LL_UNROLL>
-__device__ __noinline__ void ll_recv(float* dst, int ds, const u64* src, int ss, int rows, int n, unsigned tag, int tid, Spin& sp) {
+__device__ __forceinline__ void ll_recv(float* dst, int ds, const u64* src, int ss, int rows, int n, unsigned tag, int tid, Spin& sp,
+                                     const u64* sums = nullptr, int sr0 = 0, float inv = 0.f, float* out1 = nullptr,
+                                     float* out2 = nullptr) {
+  static_assert(MAXB <= SCAN_NW, "one warp per row of the row sums");
+  const int lane = tid & 31, wid = tid >> 5;
+  const bool has_s = sums != nullptr && wid < rows;              // warp-uniform
+  const u64* sp_row = has_s ? sums + ((size_t)(sr0 + wid) * SCAN_G + lane) * 2 : nullptr;
+  u64 sx[SCAN_G / 32], sy[SCAN_G / 32];
+  bool s_stale = has_s;
+  if (has_s)
+#pragma unroll
+    for (int i = 0; i < SCAN_G / 32; ++i) ll_load2(sp_row + 64 * i, sx[i], sy[i]);
+  // the stale partials of this lane are re-issued (true while any is stale)
+  auto poll_sums = [&]() {
+    if (!s_stale) return false;
+    bool st = false;
+#pragma unroll
+    for (int i = 0; i < SCAN_G / 32; ++i)
+      if ((unsigned)(sx[i] >> 32) != tag || (unsigned)(sy[i] >> 32) != tag) { st = true; ll_load2(sp_row + 64 * i, sx[i], sy[i]); }
+    s_stale = st;
+    return st;
+  };
   const int half = n >> 1;
   int rg = 0, kp = tid, nrg = 1, kstep = SCAN_NT;
-  if (half < SCAN_NT) { rg = tid / half; kp = tid - rg * half; nrg = SCAN_NT / half; kstep = half; if (rg >= nrg) return; }
-  for (int k = 2 * kp; k < n; k += 2 * kstep) {
-    for (int r0 = rg; r0 < rows; r0 += nrg * LL_UNROLL) {
-      u64 a[LL_UNROLL], b[LL_UNROLL];
-#pragma unroll
-      for (int u = 0; u < LL_UNROLL; ++u)
-        if (r0 + u * nrg < rows) ll_load2(src + (size_t)(r0 + u * nrg) * ss + k, a[u], b[u]);
-      // elements that came back with an old tag are re-polled TOGETHER (one L2 round trip per retry of the whole batch,
-      // not one per element)
-      for (;;) {
-        bool stale = false;
+  if (half < SCAN_NT) { rg = tid / half; kp = tid - rg * half; nrg = SCAN_NT / half; kstep = half; }
+  if (rg < nrg)
+    for (int k = 2 * kp; k < n; k += 2 * kstep) {
+      for (int r0 = rg; r0 < rows; r0 += nrg * LL_UNROLL) {
+        u64 a[LL_UNROLL], b[LL_UNROLL];
 #pragma unroll
         for (int u = 0; u < LL_UNROLL; ++u)
-          if (r0 + u * nrg < rows && ((unsigned)(a[u] >> 32) != tag || (unsigned)(b[u] >> 32) != tag)) stale = true;
-        if (!stale || sp.fail()) break;
+          if (r0 + u * nrg < rows) ll_load2(src + (size_t)(r0 + u * nrg) * ss + k, a[u], b[u]);
+        // elements that came back with an old tag are re-polled TOGETHER (one L2 round trip per retry of the whole batch,
+        // not one per element), the row-sum partials with them
+        for (;;) {
+          bool stale = false;
+#pragma unroll
+          for (int u = 0; u < LL_UNROLL; ++u)
+            if (r0 + u * nrg < rows && ((unsigned)(a[u] >> 32) != tag || (unsigned)(b[u] >> 32) != tag)) stale = true;
+          if (!stale || sp.fail()) break;
+#pragma unroll
+          for (int u = 0; u < LL_UNROLL; ++u)
+            if (r0 + u * nrg < rows && ((unsigned)(a[u] >> 32) != tag || (unsigned)(b[u] >> 32) != tag))
+              ll_load2(src + (size_t)(r0 + u * nrg) * ss + k, a[u], b[u]);
+          poll_sums();
+        }
 #pragma unroll
         for (int u = 0; u < LL_UNROLL; ++u)
-          if (r0 + u * nrg < rows && ((unsigned)(a[u] >> 32) != tag || (unsigned)(b[u] >> 32) != tag))
-            ll_load2(src + (size_t)(r0 + u * nrg) * ss + k, a[u], b[u]);
+          if (r0 + u * nrg < rows)
+            *reinterpret_cast<float2*>(dst + (r0 + u * nrg) * ds + k) =
+                make_float2(__uint_as_float((unsigned)a[u]), __uint_as_float((unsigned)b[u]));
       }
-#pragma unroll
-      for (int u = 0; u < LL_UNROLL; ++u)
-        if (r0 + u * nrg < rows)
-          *reinterpret_cast<float2*>(dst + (r0 + u * nrg) * ds + k) =
-              make_float2(__uint_as_float((unsigned)a[u]), __uint_as_float((unsigned)b[u]));
     }
+  if (!has_s) return;
+  while (poll_sums() && !sp.fail()) {}
+  float v0 = 0.f, v1 = 0.f;
+#pragma unroll
+  for (int i = 0; i < SCAN_G / 32; ++i) {
+    v0 += __uint_as_float((unsigned)sx[i]);
+    v1 += __uint_as_float((unsigned)sy[i]);
   }
+  v0 = warp_sum(v0); v1 = warp_sum(v1);
+  if (lane == 0) { out1[sr0 + wid] = v0 * inv; out2[sr0 + wid] = v1 * inv; }
 }
 
 // (row, owned-column) element a thread is responsible for during the whole scan: e = b * per_row + cj
@@ -290,7 +328,7 @@ __device__ __forceinline__ void mma_item(const float* __restrict__ X, int xs, in
 // PART[s][b][cbase + column] for all MAXB rows (every element written by exactly one lane); the caller sums the slices in
 // order (bit-reproducible).  `wbase`: first weight row; column n is row wbase + n*wst (groups of 4 columns are contiguous
 // rows).  Returns the number of slices.  No barrier inside: the caller synchronises before (X complete) and after.
-__device__ __noinline__ int product(const float* X, int xs, const float* wbase, int wst, int ngroups, int K, int B,
+__device__ __forceinline__ int product(const float* X, int xs, const float* wbase, int wst, int ngroups, int K, int B,
                                        float* PART, int ldp, int cbase, int tid) {
   if (ngroups <= 0) return 0;
   const int lane = tid & 31, wid = tid >> 5;
@@ -317,7 +355,7 @@ __device__ __forceinline__ float part_sum(const float* PART, int ldp, int ks, in
 // rows and D <= 32 classes, on the same m16n8k8 3xTF32 MMAs as `product` (rows 8..15 of the tile are unused).  Warp
 // (K slice s = wid % CLS_SLICES, class half wid / CLS_SLICES: two 8-class tiles sharing the A fragments); partials go to
 // PART[s][row][class] (fixed-order sum by the caller).
-__device__ __noinline__ void class_product(const float* X, int xs, const float* W, int wst, int D, int Kp, int nr, float* PART,
+__device__ __forceinline__ void class_product(const float* X, int xs, const float* W, int wst, int D, int Kp, int nr, float* PART,
                                               int tid) {
   const int lane = tid & 31, wid = tid >> 5, g = lane >> 2, t = lane & 3;
   const int sl = wid % CLS_SLICES, half = wid / CLS_SLICES;           // SCAN_NW == 2 * CLS_SLICES
@@ -433,7 +471,9 @@ __host__ __device__ inline GeoF make_geo_f(const Dims& a, int cta) {
   g.oX0 = o;   o += imax(mx * 4, 4);           // x_pre of the learned initial posterior z0, owned columns
   g.oPar = o;  o += g.sR + 2 * g.sDx + 2 * g.sDr;   // h0 | lnx gamma, beta | lnr gamma, beta (read every step)
   g.oMisc = o; o += 8 * MAXB + 64;           // [0,48) flags / statistics; [48,80) and [80,112) per-warp reduction scratch
-  g.oInt = o;  o += r4(64 + MAXB * 64 + 2 * SCAN_G);   // z0 class indices, z_{t-1} indices of every row, column counts (R, Dx)
+  // z0 class indices, z_{t-1} indices of every row, GRU column counts; SCAN_G more words than that, so that the
+  // shared-memory need, and with it the envelope scan_check admits, is the one of the x-statistics exchange it replaced
+  g.oInt = o;  o += r4(64 + MAXB * 64 + 2 * SCAN_G);
   g.total = o;
   return g;
 }
@@ -469,7 +509,6 @@ __global__ void __launch_bounds__(SCAN_NT, 1) rssm_scan_fwd_kernel(const b200rl_
   int* z0idx = (int*)(sm + g.oInt);
   int* zall = z0idx + 64;       // [MAXB][64] class indices of z_{t-1}, every row
   int* nctab = zall + MAXB * 64;   // valid GRU columns per CTA
-  int* nxtab = nctab + SCAN_G;     // valid x_pre columns per CTA
   const int ldp = g.ldp, xxs = imax(g.sDx, g.sDr);
   const bool sampler = g.unit_g >= 0;
   __shared__ long long sprof[32];
@@ -500,7 +539,7 @@ __global__ void __launch_bounds__(SCAN_NT, 1) rssm_scan_fwd_kernel(const b200rl_
   for (int k = tid; k < R; k += SCAN_NT) H0[k] = a.h0[k];
   for (int k = tid; k < Dx; k += SCAN_NT) { LNXG[k] = a.lnx_g[k]; LNXB[k] = a.lnx_b[k]; }
   for (int k = tid; k < Dr; k += SCAN_NT) { LNRG[k] = a.lnr_g[k]; LNRB[k] = a.lnr_b[k]; }
-  for (int c = tid; c < SCAN_G; c += SCAN_NT) { nctab[c] = owned_cols(R, c); nxtab[c] = owned_cols(Dx, c); }
+  for (int c = tid; c < SCAN_G; c += SCAN_NT) nctab[c] = owned_cols(R, c);
   for (int gi = 0; gi < g.ngx; ++gi)
     load_rows4(Win + (size_t)gi * 4 * g.kin, g.kin, 0, a.W_in, Z + A, (cta + gi * SCAN_G) * 4, Dx, 0, Z + A, g.kin, tid);
   if (wid == 0) {  // class index of the learned initial posterior (one-hot `z0`)
@@ -529,16 +568,11 @@ __global__ void __launch_bounds__(SCAN_NT, 1) rssm_scan_fwd_kernel(const b200rl_
   const int nh4 = g.ngh * 4, nh12 = g.ngh * 12, nr4 = g.ngr * 4, nx4 = g.ngx * 4;
   const Slot sH = make_slot(tid, nh4, B, cta, R);           // gate / h element
   const Slot sX = make_slot(tid, nx4, B, cta, Dx);          // x element (save of x_act)
-  const int nxcol = owned_cols(Dx, cta);                    // values per row in this CTA's share of the x LayerNorm
   const Slot sR_ = make_slot(tid, nr4, B, cta, Dr);         // rp element
   // g_pre element: c = (group, part, j) inside the row of 12*ngh products
   const int pb = nh12 > 0 ? tid / nh12 : 0, pc = tid - pb * nh12;
   const int pcol = (cta + (pc / 12) * SCAN_G) * 4 + (pc & 3), ppart = (pc % 12) >> 2;
   const bool pok = nh12 > 0 && pb < B && pcol < R;
-  float lg_g[3] = {0.f, 0.f, 0.f}, lg_b[3] = {0.f, 0.f, 0.f};
-  if (sH.ok)
-#pragma unroll
-    for (int part = 0; part < 3; ++part) { lg_g[part] = a.lng_g[part * R + sH.col]; lg_b[part] = a.lng_b[part * R + sH.col]; }
   const int ncol3 = 3 * owned_cols(R, cta);                // values per row in this CTA's share of the GRU LayerNorm
   const float bias2 = (sampler && lane < D) ? a.b_r2[g.unit_g * D + lane] : 0.f;
   float first_next = (tid < B) ? a.first[tid] : 0.f;        // is_first flags of the step about to run (threads < MAXB)
@@ -563,7 +597,7 @@ __global__ void __launch_bounds__(SCAN_NT, 1) rssm_scan_fwd_kernel(const b200rl_
 
     // ============ A (first: its hand-off is in flight while B1 runs): x_pre = W_in [z_in, a_in] for the owned columns, every row; z_in one-hot -> gather from the slice.
     // Warp b builds row b: lane = (column cj = lane / 8, part = lane % 8): 8 lanes sum S/8 gathered weights each, then a
-    // fixed 3-level shuffle tree; the row's partial LayerNorm statistics go out with the values.
+    // fixed 3-level shuffle tree.
     if (t > 0)
       for (int e = tid; e < B * S; e += SCAN_NT) {
         const int b = e / S, gq = e - b * S;
@@ -573,9 +607,6 @@ __global__ void __launch_bounds__(SCAN_NT, 1) rssm_scan_fwd_kernel(const b200rl_
     prof_mark(prof, 2, tlast, prof_on);
     for (int b = wid; b < B; b += SCAN_NW) {
       const float f = fl[b];
-      float rowv[4] = {0.f, 0.f, 0.f, 0.f};           // (lanes with part == 0) the row's x_pre of the <= 4 column groups
-      float rs = 0.f;
-      int rcnt = 0;
       for (int c0 = 0; c0 < nx4; c0 += 4) {            // 4 columns x 8 parts per pass
         const int cj = c0 + (lane >> 3), part = lane & 7;
         const int col = (cta + (cj >> 2) * SCAN_G) * 4 + (cj & 3);
@@ -595,19 +626,8 @@ __global__ void __launch_bounds__(SCAN_NT, 1) rssm_scan_fwd_kernel(const b200rl_
           const float xv = (1.f - f) * (acc + aa) + f * X0[cj];
           ll_store(ws.ll + L.x + ((size_t)par * MAXB + b) * Dx + col, xv, tag);
           a.x_pre[(row0 + b) * Dx + col] = xv;
-          rowv[c0 >> 2] = xv;
-          rs += xv;
-          ++rcnt;
         }
       }
-      // partial statistics over the owned valid columns of this row (values sit in lanes 0, 8, 16, 24)
-      rs = warp_sum(rs);
-      const float mean = nxcol > 0 ? rs / (float)nxcol : 0.f;
-      float m2 = 0.f;
-      for (int i = 0; i < 4; ++i)
-        if (i < rcnt) { const float d = rowv[i] - mean; m2 = fmaf(d, d, m2); }
-      m2 = warp_sum(m2);
-      if (lane == 0) ll_store2(ws.ll + L.sx + (((size_t)par * MAXB + b) * SCAN_G + cta) * 2, mean, m2, tag);
     }
     if (cta == (t % SCAN_G))
       for (int e = tid; e < B * A; e += SCAN_NT) a.a_in[row0 * A + e] = (1.f - fl[e / A]) * a.actions[row0 * A + e];
@@ -628,56 +648,22 @@ __global__ void __launch_bounds__(SCAN_NT, 1) rssm_scan_fwd_kernel(const b200rl_
     const float hin = sH.ok ? Xh[sH.b * g.sR + sH.col] : 0.f;
     prof_mark(prof, 13, tlast, prof_on);
 
-    // ============ B2: x-part of the GRU product; g_pre columns; partial LayerNorm statistics
+    // ============ B2: x = SiLU(LN(x_pre)), x-part of the GRU product; g_pre columns; partial LayerNorm statistics
     ll_recv<8>(Xx, xxs, ws.ll + L.x + (size_t)par * MAXB * Dx, Dx, B, Dx, tag, tid, sp);
-    for (int b = wid; b < B; b += SCAN_NW) {               // merge the x LayerNorm statistics of row b (Chan)
-      float pm[SCAN_G / 32], pq[SCAN_G / 32];
-      u64 x[SCAN_G / 32], y[SCAN_G / 32];
-#pragma unroll
-      for (int i = 0; i < SCAN_G / 32; ++i)
-        ll_load2(ws.ll + L.sx + (((size_t)par * MAXB + b) * SCAN_G + lane + 32 * i) * 2, x[i], y[i]);
-      for (;;) {                                   // stale partials are re-polled together
-        bool stale = false;
-#pragma unroll
-        for (int i = 0; i < SCAN_G / 32; ++i)
-          if ((unsigned)(x[i] >> 32) != tag || (unsigned)(y[i] >> 32) != tag) stale = true;
-        if (!stale || sp.fail()) break;
-#pragma unroll
-        for (int i = 0; i < SCAN_G / 32; ++i)
-          if ((unsigned)(x[i] >> 32) != tag || (unsigned)(y[i] >> 32) != tag)
-            ll_load2(ws.ll + L.sx + (((size_t)par * MAXB + b) * SCAN_G + lane + 32 * i) * 2, x[i], y[i]);
-      }
-#pragma unroll
-      for (int i = 0; i < SCAN_G / 32; ++i) {
-        pm[i] = __uint_as_float((unsigned)x[i]);
-        pq[i] = __uint_as_float((unsigned)y[i]);
-      }
-      float sm_ = 0.f;
-#pragma unroll
-      for (int i = 0; i < SCAN_G / 32; ++i) sm_ += (float)nxtab[lane + 32 * i] * pm[i];
-      const float mean = warp_sum(sm_) / (float)Dx;
-      float m2 = 0.f;
-#pragma unroll
-      for (int i = 0; i < SCAN_G / 32; ++i) {
-        const float d = pm[i] - mean;
-        m2 += pq[i] + (float)nxtab[lane + 32 * i] * d * d;
-      }
-      m2 = warp_sum(m2);
-      if (lane == 0) {
-        const float rstd = rsqrtf(m2 / (float)Dx + a.eps);
-        misc[16 + b] = mean;
-        misc[32 + b] = rstd;
-        if (cta == ((t + 1) % SCAN_G)) {
-          ws.ln_stats[((size_t)0 * NB + row0 + b) * 2] = mean;
-          ws.ln_stats[((size_t)0 * NB + row0 + b) * 2 + 1] = rstd;
-        }
-      }
-    }
     __syncthreads();
-    for (int k = tid; k < Dx; k += SCAN_NT) {              // x = SiLU(LN(x_pre)) in place, every row (column k per thread)
-      const float gk = LNXG[k], bk = LNXB[k];
-      for (int b = 0; b < B; ++b)
-        Xx[b * xxs + k] = fsilu((Xx[b * xxs + k] - misc[16 + b]) * misc[32 + b] * gk + bk);
+    for (int b = wid; b < B; b += SCAN_NW) {   // warp b normalises row b in place: centred two passes, fixed order
+      float* xr = Xx + b * xxs;
+      float s = 0.f;
+      for (int k = lane; k < Dx; k += 32) s += xr[k];
+      const float mean = warp_sum(s) / (float)Dx;
+      float m2 = 0.f;
+      for (int k = lane; k < Dx; k += 32) { const float d = xr[k] - mean; m2 = fmaf(d, d, m2); }
+      const float rstd = rsqrtf(warp_sum(m2) / (float)Dx + a.eps);
+      for (int k = lane; k < Dx; k += 32) xr[k] = fsilu((xr[k] - mean) * rstd * LNXG[k] + LNXB[k]);
+      if (lane == 0 && cta == ((t + 1) % SCAN_G)) {
+        ws.ln_stats[((size_t)0 * NB + row0 + b) * 2] = mean;
+        ws.ln_stats[((size_t)0 * NB + row0 + b) * 2 + 1] = rstd;
+      }
     }
     __syncthreads();
     if (sX.ok) a.x_act[(row0 + sX.b) * Dx + sX.col] = Xx[sX.b * xxs + sX.col];
@@ -705,7 +691,12 @@ __global__ void __launch_bounds__(SCAN_NT, 1) rssm_scan_fwd_kernel(const b200rl_
     if (pok) a.g_pre[(row0 + pb) * 3 * R + ppart * R + pcol] = gpre;      // save after the hand-off
     prof_mark(prof, 5, tlast, prof_on);
 
-    // ============ C: merge statistics (Chan), LayerNorm, GRU gate -> h_t for the owned columns
+    // ============ C: merge statistics (Chan), LayerNorm, GRU gate -> h_t for the owned columns.  The element's LayerNorm
+    // parameters are loaded here, in flight during the wait (kept in registers across the whole step, they were spilled)
+    float lg_g[3] = {0.f, 0.f, 0.f}, lg_b[3] = {0.f, 0.f, 0.f};
+    if (sH.ok)
+#pragma unroll
+      for (int part = 0; part < 3; ++part) { lg_g[part] = a.lng_g[part * R + sH.col]; lg_b[part] = a.lng_b[part * R + sH.col]; }
     for (int b0 = wid; b0 < B; b0 += 2 * SCAN_NW) {          // a warp merges up to two rows, all their loads in flight
       u64 x[2][SCAN_G / 32], y[2][SCAN_G / 32];
 #pragma unroll
@@ -946,51 +937,8 @@ __host__ __device__ inline GeoB make_geo_b(const Dims& a, int cta) {
   return g;
 }
 
-// (sum dxh, sum dxh*xh) / n of the rows [r0, r0+nr) from the per-CTA partials; one warp per row (two rows in flight per
-// warp), fixed summation order
-__device__ __noinline__ void recv_row_sums(const u64* base, int par, int r0, int nr, unsigned tag, float inv, float* out1,
-                                              float* out2, int tid, Spin& sp) {
-  const int lane = tid & 31, wid = tid >> 5;
-  for (int bb0 = wid; bb0 < nr; bb0 += 2 * SCAN_NW) {
-    u64 x[2][SCAN_G / 32], y[2][SCAN_G / 32];
-#pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      const int bb = bb0 + rr * SCAN_NW;
-      if (bb < nr)
-#pragma unroll
-        for (int i = 0; i < SCAN_G / 32; ++i)
-          ll_load2(base + (((size_t)par * MAXB + r0 + bb) * SCAN_G + lane + 32 * i) * 2, x[rr][i], y[rr][i]);
-    }
-#pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      const int bb = bb0 + rr * SCAN_NW;
-      if (bb >= nr) continue;
-      const int b = r0 + bb;
-      float v0 = 0.f, v1 = 0.f;
-      for (;;) {                                   // stale partials are re-polled together
-        bool stale = false;
-#pragma unroll
-        for (int i = 0; i < SCAN_G / 32; ++i)
-          if ((unsigned)(x[rr][i] >> 32) != tag || (unsigned)(y[rr][i] >> 32) != tag) stale = true;
-        if (!stale || sp.fail()) break;
-#pragma unroll
-        for (int i = 0; i < SCAN_G / 32; ++i)
-          if ((unsigned)(x[rr][i] >> 32) != tag || (unsigned)(y[rr][i] >> 32) != tag)
-            ll_load2(base + (((size_t)par * MAXB + b) * SCAN_G + lane + 32 * i) * 2, x[rr][i], y[rr][i]);
-      }
-#pragma unroll
-      for (int i = 0; i < SCAN_G / 32; ++i) {
-        v0 += __uint_as_float((unsigned)x[rr][i]);
-        v1 += __uint_as_float((unsigned)y[rr][i]);
-      }
-      v0 = warp_sum(v0); v1 = warp_sum(v1);
-      if (lane == 0) { out1[b] = v0 * inv; out2[b] = v1 * inv; }
-    }
-  }
-}
-
 // per-row sums of the staged (dxh, dxh*xh) pairs of this CTA's columns -> LL partial for every row
-__device__ __noinline__ void send_row_sums(const float* ST, int ncols, int B, u64* base, int par, int cta, unsigned tag, int tid) {
+__device__ __forceinline__ void send_row_sums(const float* ST, int ncols, int B, u64* base, int par, int cta, unsigned tag, int tid) {
   const int lane = tid & 31, wid = tid >> 5;
   for (int b = wid; b < B; b += SCAN_NW) {
     float s1 = 0.f, s2 = 0.f;
@@ -1146,8 +1094,8 @@ rssm_scan_bwd_kernel(const b200rl_rssm_scan_args a, const b200rl_rssm_scan_grads
     if (unit) {
       const int gq = g.unit_g, nr = g.unit_nr, rb = g.unit_r0;
       if (!last) {
-        ll_recv<4>(X, xw, ws.ll + L.d + ((size_t)(par ^ 1) * MAXB + rb) * Dx, Dx, nr, Dx, (unsigned)bt, tid, sp);
-        recv_row_sums(ws.ll + L.sd, par ^ 1, rb, nr, (unsigned)bt, 1.f / (float)Dx, S1, S2, tid, sp);
+        ll_recv<4>(X, xw, ws.ll + L.d + ((size_t)(par ^ 1) * MAXB + rb) * Dx, Dx, nr, Dx, (unsigned)bt, tid, sp,
+                   ws.ll + L.sd + (size_t)(par ^ 1) * MAXB * SCAN_G * 2, rb, 1.f / (float)Dx, S1, S2);
         __syncthreads();
         prof_mark(prof, 17, tlast, prof_on);
         class_product(X, xw, WinU, g.winst, D, g.sDx, nr, PART, tid);
@@ -1219,8 +1167,8 @@ rssm_scan_bwd_kernel(const b200rl_rssm_scan_args a, const b200rl_rssm_scan_grads
 
     // ============ R: dh = d_latent_h + carry + d_rp_pre W_r1h ; GRU gate backward ; dxh of the GRU LayerNorm
     __syncthreads();
-    ll_recv<4>(X, xw, ws.ll + L.b + (size_t)par * MAXB * Dr, Dr, B, Dr, tag, tid, sp);
-    recv_row_sums(ws.ll + L.sb, par, 0, B, tag, 1.f / (float)Dr, S1, S2, tid, sp);
+    ll_recv<4>(X, xw, ws.ll + L.b + (size_t)par * MAXB * Dr, Dr, B, Dr, tag, tid, sp,
+               ws.ll + L.sb + (size_t)par * MAXB * SCAN_G * 2, 0, 1.f / (float)Dr, S1, S2);
     __syncthreads();
     prof_mark(prof, 21, tlast, prof_on);
     const int ks1 = product(X, xw, W1T, g.sDr, g.ngh, Dr, B, PART, ldp, 0, tid);
@@ -1274,8 +1222,8 @@ rssm_scan_bwd_kernel(const b200rl_rssm_scan_args a, const b200rl_rssm_scan_grads
     float acc_h = sH.ok ? part_sum(PART, ldp, ksa, sH.b, sH.cj) : 0.f;
     float acc_x = sX.ok ? part_sum(PART, ldp, ksa, sX.b, nh4 + sX.cj) : 0.f;
     __syncthreads();
-    ll_recv<4>(X, xw, ws.ll + L.c + (size_t)par * MAXB * 3 * R + (size_t)2 * R, 3 * R, B, R, tag, tid, sp);
-    recv_row_sums(ws.ll + L.sc, par, 0, B, tag, 1.f / (float)(3 * R), S1, S2, tid, sp);
+    ll_recv<4>(X, xw, ws.ll + L.c + (size_t)par * MAXB * 3 * R + (size_t)2 * R, 3 * R, B, R, tag, tid, sp,
+               ws.ll + L.sc + (size_t)par * MAXB * SCAN_G * 2, 0, 1.f / (float)(3 * R), S1, S2);
     __syncthreads();
     const int ksb = product(X, xw, WgT + 2 * g.sR, g.wgst, g.ngh + g.ngx, R, B, PART, ldp, 0, tid);
     __syncthreads();
@@ -1418,7 +1366,7 @@ __host__ __device__ inline GeoG make_geo_g(int R, int cta, bool backward) {
 
 // Merges the per-CTA (mean, M2) partials of one row's LayerNorm statistics (Chan); the whole warp works on the row.
 // `cnt[c]`: values CTA c contributed, `n` their total.
-__device__ __noinline__ void merge_row_stats(const u64* base, unsigned tag, const int* cnt, float n, float eps, int lane,
+__device__ __forceinline__ void merge_row_stats(const u64* base, unsigned tag, const int* cnt, float n, float eps, int lane,
                                                 Spin& sp, float& mean, float& rstd) {
   u64 x[SCAN_G / 32], y[SCAN_G / 32];
 #pragma unroll
@@ -1674,9 +1622,14 @@ gru_scan_bwd_kernel(const b200rl_gru_scan_args a, const b200rl_gru_scan_grads q)
     // ============ dh_in = d_g_pre W_g[:, :R] for the owned columns (K = 3R, in 3 / pw passes)
     float acc_h = 0.f;
     for (int p0 = 0; p0 < 3; p0 += g.pw) {
-      for (int part = p0; part < p0 + g.pw; ++part)
-        ll_recv<4>(X + (part - p0) * g.sR, xw, ll + L.c + (size_t)par * MAXB * 3 * R + (size_t)part * R, 3 * R, B, R, tag, tid, sp);
-      if (p0 == 0) recv_row_sums(ll + L.sc, par, 0, B, tag, 1.f / (float)(3 * R), S1, S2, tid, sp);
+      for (int part = p0; part < p0 + g.pw; ++part) {
+        const u64* src = ll + L.c + (size_t)par * MAXB * 3 * R + (size_t)part * R;
+        if (part == g.pw - 1)        // the row sums ride with the last part of the first pass
+          ll_recv<4>(X + (part - p0) * g.sR, xw, src, 3 * R, B, R, tag, tid, sp, ll + L.sc + (size_t)par * MAXB * SCAN_G * 2, 0,
+                     1.f / (float)(3 * R), S1, S2);
+        else
+          ll_recv<4>(X + (part - p0) * g.sR, xw, src, 3 * R, B, R, tag, tid, sp);
+      }
       __syncthreads();
       const int ks = product(X, xw, WgT + p0 * g.sR, wgst, g.ngh, g.pw * g.sR, B, PART, ldp, 0, tid);
       __syncthreads();
