@@ -329,6 +329,39 @@ def uniform_mix64(x: Tensor, unimix: float) -> Tensor:
     return torch.log(probs.clamp(FP32_EPS, 1 - FP32_EPS))
 
 
+def unimix_fwd_err(x64: Tensor, unimix: float):
+    """The unimix mix of the logits x64 [..., K] as an fp32 kernel forms it, with the error of each step:
+    (s, E_s, pm, E_pm, l, E_l): s = softmax(x) with relative error E_s, pm = (1 - unimix) s + unimix / K with relative
+    error E_pm (None, None without unimix), l = log(clamp(pm)) (x itself without unimix) with absolute error E_l.
+    The clamp is continuous, so it passes pm's relative error on unchanged."""
+    K = x64.shape[-1]
+    s, E_s = x64.softmax(-1), _softmax_rel(x64)
+    if unimix <= 0:
+        return s, E_s, None, None, x64, torch.zeros_like(x64)
+    pm = (1 - unimix) * s + unimix / K
+    E_pm = ((1 - unimix) * s * (E_s + 2 * U) + 2 * U * unimix / K) / pm + U
+    l = torch.log(pm.clamp(FP32_EPS, 1 - FP32_EPS))
+    return s, E_s, pm, E_pm, l, E_pm + 2 * U * l.abs()
+
+
+def unimix_bwd_err(s: Tensor, E_s: Tensor, pm: Tensor, E_pm: Tensor, gg: Tensor, E_gg: Tensor, unimix: float):
+    """The chain rule through the unimix mix and its clamp: the gradient gg w.r.t. l = log(clamp(pm)) (error E_gg)
+    taken to the logits, dr = s (ds - sum s ds) with ds = gg (1 - unimix) / pm inside the clamp and 0 outside.
+    Returns (dr, bound of its error).  A kernel decides "inside" from its fp32 pm: an element whose float64 pm lies
+    within its error of either clamp edge may take either branch, so its ds may also be the other branch's."""
+    inside = ((pm >= FP32_EPS) & (pm <= 1 - FP32_EPS)).double()
+    slack = E_pm * pm
+    edge = (((pm - FP32_EPS).abs() <= slack) | ((pm - (1 - FP32_EPS)).abs() <= slack)).double()
+    ds = inside * gg * (1 - unimix) / pm
+    E_ds = (inside * (E_gg + gg.abs() * (E_pm + 3 * U))
+            + edge * (gg.abs() + E_gg) * (1 + E_pm + 3 * U)) * (1 - unimix) / pm
+    sds = (s * ds).sum(-1, keepdim=True)
+    E_sds = (s * E_ds + (s * ds).abs() * (E_s + U)).sum(-1, keepdim=True) \
+        + tau1(s.shape[-1]) * (s * ds).abs().sum(-1, keepdim=True)
+    dr = s * (ds - sds)
+    return dr, s * (E_ds + E_sds) + dr.abs() * (E_s + U) + (U * s + TINY) * (ds - sds).abs()
+
+
 def actor_loss(raw: Tensor, actions: Tensor, lam: Tensor, val: Tensor, discount: Tensor, moments_: Tensor,
                head_dims: Sequence[int], unimix: float, ent_coef: float, scale: float):
     """The discrete objective of dreamer_v3.py: rows[m] = discount (sum_heads log_prob(action) adv + ent_coef sum_heads
@@ -361,16 +394,7 @@ def actor_loss(raw: Tensor, actions: Tensor, lam: Tensor, val: Tensor, discount:
     gs = (scale * D).abs().unsqueeze(-1)
     heads = []
     for o, K, idx in per_head:
-        xh = x.detach()[:, o:o + K]
-        s = xh.softmax(-1)
-        E_s = _softmax_rel(xh)
-        if unimix > 0:
-            pm = (1 - unimix) * s + unimix / K
-            E_pm = ((1 - unimix) * s * (E_s + 2 * U) + 2 * U * unimix / K) / pm + U
-            l = torch.log(pm.clamp(FP32_EPS, 1 - FP32_EPS))
-            E_l = E_pm + 2 * U * l.abs()
-        else:
-            l, E_l = xh, torch.zeros_like(xh)
+        s, E_s, pm, E_pm, l, E_l = unimix_fwd_err(x.detach()[:, o:o + K], unimix)
         lg = l - torch.logsumexp(l, -1, keepdim=True)
         p = lg.exp()
         E_lg = E_l + lse_err(l) + (p * E_l).sum(-1, keepdim=True) + U * lg.abs()
@@ -382,8 +406,7 @@ def actor_loss(raw: Tensor, actions: Tensor, lam: Tensor, val: Tensor, discount:
         E_obj += E_lg.gather(1, idx.unsqueeze(-1)).squeeze(-1) * adv.abs() + logp.abs() * E_adv \
             + 2 * U * (logp * adv).abs()
         E_ent_tot += E_ent.squeeze(-1)
-        heads.append((o, K, idx, s, E_s, l, lg, p, E_lg, e_p, hent, E_ent, pm if unimix > 0 else None,
-                      E_pm if unimix > 0 else None))
+        heads.append((o, K, idx, s, E_s, l, lg, p, E_lg, e_p, hent, E_ent, pm, E_pm))
     for o, K, idx, s, E_s, l, lg, p, E_lg, e_p, hent, E_ent, pm, E_pm in heads:
         dl = F.one_hot(idx, K).double() - p
         a1 = adv.unsqueeze(-1)
@@ -394,14 +417,7 @@ def actor_loss(raw: Tensor, actions: Tensor, lam: Tensor, val: Tensor, discount:
                      + 4 * U * ((a1 * dl).abs() + abs(ent_coef) * dent.abs())
                      + TINY * (a1.abs() + abs(ent_coef) * ((lg + hent).abs() + 1))) + 2 * U * gg.abs()
         if unimix > 0:
-            inside = ((pm >= FP32_EPS) & (pm <= 1 - FP32_EPS)).double()
-            ds = inside * gg * (1 - unimix) / pm
-            E_ds = inside * (E_gg + gg.abs() * (E_pm + 3 * U)) * (1 - unimix) / pm
-            sds = (s * ds).sum(-1, keepdim=True)
-            E_sds = (s * E_ds + (s * ds).abs() * (E_s + U)).sum(-1, keepdim=True) \
-                + tau1(K) * (s * ds).abs().sum(-1, keepdim=True)
-            dr = s * (ds - sds)
-            b_draw[:, o:o + K] = s * (E_ds + E_sds) + dr.abs() * (E_s + U) + (U * s + TINY) * (ds - sds).abs()
+            b_draw[:, o:o + K] = unimix_bwd_err(s, E_s, pm, E_pm, gg, E_gg, unimix)[1]
         else:
             b_draw[:, o:o + K] = E_gg
     b_rows = D.abs() * (E_obj + abs(ent_coef) * E_ent_tot
