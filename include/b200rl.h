@@ -7,7 +7,8 @@
  *
  * Conventions
  *   - plain pointers + sizes only; every pointer is a DEVICE pointer owned by the caller (borrowed);
- *     nothing is allocated or freed by the library; no host synchronisation; all work is enqueued on
+ *     nothing is allocated or freed by the library but its split-K and deterministic-mode partials pools (grown
+ *     outside stream capture only); no host synchronisation; all work is enqueued on
  *     `stream` (pass the caller's current stream) — hence CUDA-graph capturable;
  *   - fp32, row-major; `ld*` = row stride in elements of a 2-D view whose inner stride is 1;
  *   - return 0 on success; non-zero => b200rl_last_error() (thread-local message);
@@ -46,6 +47,17 @@ int b200rl_gemm_f32(const float* A, const float* B, float* C, const float* bias,
  * both precisions against a float64 reference (tests/test_gpu_tc_precision.py). */
 int b200rl_set_matmul_precision(int tf32_passes);
 int b200rl_get_matmul_precision(void);
+/* Deterministic mode, process-wide like torch.use_deterministic_algorithms (0 = off, the default; 1 = on).  When on,
+ * every reduction that otherwise adds float partials with atomics (sumsq, col_sum, the LayerNorm parameter gradients,
+ * the SIMT and batched split-K products, the convolution weight gradients) writes one partial per CTA or warp to a slot
+ * and adds the slots in a fixed order: the same inputs give bit-identical outputs on the same GPU type.  The slots live
+ * in a library-owned pool, per device, that grows outside stream capture (run a step eagerly before capturing it); no
+ * launch reads what the pool held before. */
+int b200rl_set_deterministic(int on);
+int b200rl_get_deterministic(void);
+/* fills the current device's deterministic-mode pool with `byte` (0xFF: NaN in every float and double slot), so a
+ * test can show that no deterministic launch reads a slot it has not written; no-op before the pool exists */
+int b200rl_deterministic_pool_fill(int byte, cudaStream_t stream);
 int b200rl_gemm_tc_supported(const float* A, const float* B, int M, int N, int K, int lda, int ldb, int transA,
                              int transB);
 int b200rl_gemm_tc(const float* A, const float* B, float* C, const float* bias, int M, int N, int K, int lda, int ldb,

@@ -18,6 +18,7 @@ import torch
 
 from sheeprl_b200.algos.dreamer_v3.dreamer_v3 import B200Adam
 from sheeprl_b200.algos.ppo.engine import PPOEngine
+from sheeprl_b200.lib import sync_deterministic
 
 INT32_MAX = 2 ** 31 - 1
 
@@ -51,6 +52,7 @@ class A2CEngine(PPOEngine):
         index_batches: the row indices of each minibatch, in sampler order.  `on_minibatch(losses[3])` is called once
         per minibatch with its (policy, value, entropy) losses."""
         o, s, hp = self.ops, self.spec, self.hp
+        sync_deterministic(o)
         batches = [list(ib) for ib in index_batches]
         B, N = self._check_rows([len(ib) for ib in batches])
         idx = torch.as_tensor([i for ib in batches for i in ib], dtype=torch.int64).to(self.device, non_blocking=True)

@@ -12,6 +12,7 @@ from typing import Any, Dict, Optional, Sequence
 import torch
 
 from sheeprl_b200.engine import DV3Engine
+from sheeprl_b200.lib import sync_deterministic
 from sheeprl_b200.utils.registry import register_algorithm
 
 METRIC_ORDER = (
@@ -136,6 +137,7 @@ def train(
         raise ValueError("is_continuous differs from the value build_agent() was called with")
     if moments is not None and getattr(moments, "low", None) is not None and moments.low.data_ptr() != eng.moments_state.data_ptr():
         moments.bind(eng.moments_state)
+    sync_deterministic(eng.ops)        # before the graph key, which holds the mode
     if noise is None and eng.use_cuda_graph():
         # the whole update as one CUDA-graph replay (sheeprl_b200/graph.py): the batch is copied into the graph's static
         # inputs; the reference's in-place `data["is_first"][0] = 1` (dreamer_v3.py:100) still reaches the caller's tensor

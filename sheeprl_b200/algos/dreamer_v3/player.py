@@ -18,6 +18,7 @@ from typing import Dict, Optional, Sequence
 import torch
 
 from sheeprl_b200.engine import ACT_SILU, DV3Engine
+from sheeprl_b200.lib import sync_deterministic
 
 
 class PlayerDV3:
@@ -101,6 +102,7 @@ class PlayerDV3:
         `mask` is ignored, as the reference's `Actor.forward` ignores it (the reference's `test()` passes the observation's
         `mask*` keys, an empty dict for environments without them)."""
         e, ops, E = self.eng, self.eng.ops, self.num_envs
+        sync_deterministic(ops)
         Z = e.Z
         if e.has_cnn:
             x = e.image_batch(obs, E)

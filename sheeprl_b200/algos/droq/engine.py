@@ -20,6 +20,7 @@ import torch
 
 from sheeprl_b200.algos.sac.engine import SACEngine
 from sheeprl_b200.dense import DropoutLayerNormReLU
+from sheeprl_b200.lib import sync_deterministic
 
 LN_EPS = 1e-5                  # nn.LayerNorm(H) (droq/agent.py:40-42)
 MASKS_PER_STEP = 4             # target layer 0, 1; online layer 0, 1 (each [n, B, ceil(H/32)] words)
@@ -100,6 +101,7 @@ class DroQEngine(SACEngine):
         dropout call order: per minibatch the target critics' two layers, then the online critics', then the policy
         loss's."""
         o, O, B = self.ops, self.O, self.B
+        sync_deterministic(o)
         rows = critic_data["observations"].shape[0]
         if rows % B or actor_obs.shape != (B, O):
             raise ValueError(f"critic rows {rows} must be a multiple of the batch size {B}; actor rows {tuple(actor_obs.shape)}")

@@ -26,6 +26,7 @@ from typing import Dict, Optional, Sequence
 import torch
 
 from sheeprl_b200.engine import TWOHOT_HIGH, TWOHOT_LOW, DV3Engine, _MLP, dv3_param_shapes
+from sheeprl_b200.lib import sync_deterministic
 from sheeprl_b200.params import FlatGroup
 
 
@@ -146,6 +147,7 @@ class P2EDV3Engine(DV3Engine):
     def train_step(self, data: Dict[str, torch.Tensor], noise: Optional[Dict[str, torch.Tensor]] = None):
         """noise (parity mode): {"post", "img_state_expl", "img_action_expl", "img_state_task", "img_action_task"}"""
         ops = self.ops
+        sync_deterministic(ops)
         N, H, Z = self.N, self.H, self.Z
         if noise is None:
             self._draw_noise(None)                                                   # post / task rollout streams 0-2

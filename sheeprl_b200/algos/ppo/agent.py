@@ -10,6 +10,7 @@ from typing import Any, Dict, Optional, Sequence, Tuple
 import torch
 
 from sheeprl_b200.algos.ppo.engine import PPOEngine
+from sheeprl_b200.lib import sync_deterministic
 
 
 def spec_from_cfg(cfg, actions_dim: Sequence[int], is_continuous: bool, obs_space) -> dict:
@@ -150,6 +151,7 @@ class PPOPlayer:
 
     def _run(self, obs, actor: bool, critic: bool):
         e, s = self.engine, self.engine.spec
+        sync_deterministic(e.ops)
         rgb, x_state = gather_obs(s, obs)
         normalized = False
         if rgb is not None:

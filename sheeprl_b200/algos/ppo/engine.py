@@ -22,6 +22,7 @@ from typing import Dict, Optional, Sequence
 import torch
 
 from sheeprl_b200.dense import Act, LayerNormAct, Linear, Stack
+from sheeprl_b200.lib import sync_deterministic
 from sheeprl_b200.params import FlatGroup
 
 CONVS = ((8, 4, 32), (4, 2, 64), (3, 1, 64))        # NatureCNN (kernel, stride, channels) models.py:301-309
@@ -326,6 +327,7 @@ class PPOEngine:
                            **g.adam_kwargs(self.opt.get("weight_decay", 0.0)))
 
     def train(self, data: Dict[str, torch.Tensor], index_batches: Sequence[Sequence[int]], on_minibatch=None):
+        sync_deterministic(self.ops)
         for ib in index_batches:
             idx = torch.as_tensor(ib, dtype=torch.int64).to(self.device, non_blocking=True)
             self.minibatch_step(data, idx)

@@ -11,6 +11,7 @@ import torch
 
 from sheeprl_b200.algos.ppo.agent import PPOPlayer, default_init, gather_obs, hp_from_cfg, spec_from_cfg
 from sheeprl_b200.algos.ppo_recurrent.engine import RecurrentPPOEngine
+from sheeprl_b200.lib import sync_deterministic
 
 
 def rnn_spec_from_cfg(cfg) -> dict:
@@ -99,6 +100,7 @@ class RecurrentPPOPlayer(PPOPlayer):
         if mask is not None:
             raise NotImplementedError("the player steps one time step per call; mask is not supported")
         e = self.engine
+        sync_deterministic(e.ops)
         rgb, x_state = gather_obs(e.spec, obs)
         E = prev_actions.shape[-2]
         H = e.H

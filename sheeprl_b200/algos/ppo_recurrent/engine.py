@@ -26,6 +26,7 @@ import torch
 
 from sheeprl_b200.algos.ppo.engine import PPOEngine
 from sheeprl_b200.dense import Act, LayerNormAct, Linear, Stack
+from sheeprl_b200.lib import sync_deterministic
 
 RNN_LN_EPS = 1e-3                                     # RecurrentModel's pre/post MLP LayerNorm (agent.py:31-35, 52-56)
 
@@ -231,6 +232,7 @@ class RecurrentPPOEngine(PPOEngine):
 
     def train(self, data: Dict[str, torch.Tensor], index_batches: Sequence[Sequence[int]], on_minibatch=None,
               prepared: Optional[dict] = None):
+        sync_deterministic(self.ops)
         d = prepared if prepared is not None else self.prepare(data)
         for ib in index_batches:
             seqs = torch.as_tensor(ib, dtype=torch.int64).to(self.device, non_blocking=True)

@@ -14,6 +14,7 @@ from typing import Any, Dict, Optional, Tuple
 import torch
 
 from sheeprl_b200.algos.sac.engine import SACEngine
+from sheeprl_b200.lib import sync_deterministic
 
 
 def _default_linear_init(shapes, generator: torch.Generator) -> Dict[str, torch.Tensor]:
@@ -94,6 +95,7 @@ class SACPlayer:
     @torch.no_grad()
     def get_actions(self, obs: torch.Tensor, greedy: bool = False) -> torch.Tensor:
         e, o = self.engine, self.engine.ops
+        sync_deterministic(o)
         x = obs.reshape(-1, e.O).float().contiguous()
         E = x.shape[0]
         if E not in self._bufs:

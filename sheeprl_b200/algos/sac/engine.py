@@ -20,6 +20,7 @@ from typing import Dict, Optional
 import torch
 
 from sheeprl_b200.dense import Act, Linear, Stack, stacked
+from sheeprl_b200.lib import sync_deterministic
 from sheeprl_b200.params import FlatGroup
 
 
@@ -137,6 +138,7 @@ class SACEngine:
         """data: observations / next_observations [B,O], actions [B,A], rewards / terminated [B,1] (float32, on the
         device).  noise (parity tests): {"eps_next", "eps_cur"} N(0,1) draws of the two rsample calls."""
         o, O = self.ops, self.O
+        sync_deterministic(o)
         obs, nobs = data["observations"], data["next_observations"]
         assert obs.shape == (self.B, O) and data["actions"].shape == (self.B, self.A), (obs.shape, data["actions"].shape)
         if noise is None:

@@ -94,3 +94,10 @@ __device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint
 }
 
 static inline int ceil_div(long long a, long long b) { return (int)((a + b - 1) / b); }
+
+// Deterministic mode (det.cu): the launchers of the float-atomic reductions read det_mode() and, when it is set, write
+// per-CTA partials to slots of det_workspace() that det_sum_slots adds in slot order (out += sum).
+bool det_mode();
+int det_workspace(size_t bytes, cudaStream_t st, void** ws);
+int det_sum_slots(const float* part, int slots, long long n, float* out_a, long long na, float* out_b, cudaStream_t st);
+int det_sum_slots_d(const double* part, int slots, double* out, cudaStream_t st);

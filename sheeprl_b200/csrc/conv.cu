@@ -183,6 +183,8 @@ conv_igemm_kernel(const float* __restrict__ In, const float* __restrict__ W, flo
 }
 
 // dW[cs,cb,tap] += sum_m small[m,cs] * big[row(m,tap),cb]; 64x64 (cs x cb) tiles, 16 pixel rows per k-step.
+// DET: dW is a slot array of Cs*Cb*16 floats per split; the CTA stores its tile to slot `split` (det_sum_slots adds them).
+template <bool DET>
 __global__ void __launch_bounds__(256)
 conv_wgrad_kernel(const float* __restrict__ Small, const float* __restrict__ Big, float* __restrict__ dW, int NB,
                   int h, int w, int Cs, int Cb, long long rows_per_split) {
@@ -258,14 +260,16 @@ conv_wgrad_kernel(const float* __restrict__ Small, const float* __restrict__ Big
     for (int j = 0; j < 4; ++j) {
       const int cb = cb0 + tx * 4 + j;
       if (cb >= Cb) continue;
-      atomicAdd(&dW[((long long)cs * Cb + cb) * 16 + tap], acc[i][j]);
+      if constexpr (DET) dW[((long long)split * Cs + cs) * Cb * 16 + (long long)cb * 16 + tap] = acc[i][j];
+      else atomicAdd(&dW[((long long)cs * Cb + cb) * 16 + tap], acc[i][j]);
     }
   }
 }
 
 // Weight gradient when the big image has very few channels (RGB input / output layers): all 16*CB
 // (tap, channel) columns of a pixel are staged once and shared by every small-image channel.
-template <int CB>
+// DET: dW is a slot array of Cs*CB*16 floats per CTA; the CTA stores its partials to slot blockIdx.x.
+template <int CB, bool DET>
 __global__ void __launch_bounds__(256)
 conv_wgrad_smallcb_kernel(const float* __restrict__ Small, const float* __restrict__ Big, float* __restrict__ dW,
                           int NB, int h, int w, int Cs, long long rows_per_block) {
@@ -322,7 +326,8 @@ conv_wgrad_smallcb_kernel(const float* __restrict__ Small, const float* __restri
     if (o < nout) {
       const int cs = o % Cs, q = o / Cs;
       const int tap = q / CB, c = q - tap * CB;
-      atomicAdd(&dW[((long long)cs * CB + c) * 16 + tap], acc[i]);
+      if constexpr (DET) dW[((long long)blockIdx.x * Cs + cs) * CB * 16 + c * 16 + tap] = acc[i];
+      else atomicAdd(&dW[((long long)cs * CB + c) * 16 + tap], acc[i]);
     }
   }
 }
@@ -598,26 +603,51 @@ extern "C" int b200rl_conv_wgrad(const float* small, const float* big, float* dW
   if (!accumulate) RL_CUDA(cudaMemsetAsync(dW, 0, sizeof(float) * (size_t)Cs * Cb * 16, st));
   if (b200rl_thin_wgrad_supported(Cs, Cb)) return b200rl_conv_wgrad_thin(small, big, dW, NB, h, w, Cs, Cb, st);
   const long long Mtot = (long long)NB * h * w;
+  const long long nW = (long long)Cs * Cb * 16;
+  // deterministic mode: per-split (per-CTA) partials in slots of nW floats, added to dW in slot order
+  const bool det = det_mode();
+  float* part = nullptr;
+  auto slots_ws = [&](long long slots) -> int {
+    void* ws = nullptr;
+    if (int rc = det_workspace(sizeof(float) * nW * slots, st, &ws)) return rc;
+    part = static_cast<float*>(ws);
+    return B200RL_OK;
+  };
   if (Cb <= 4 && Cs * 16 * Cb <= 24 * 256) {
     long long blocks = min((long long)4 * kNumSMs, (Mtot + 31) / 32);
     long long rpb = ((Mtot + blocks - 1) / blocks + 31) / 32 * 32;
     blocks = (Mtot + rpb - 1) / rpb;
     const size_t smem = sizeof(float) * 32 * (Cs + 16 * Cb);
+#define WGRAD_SMALLCB(CB_)                                                                                           \
+  do {                                                                                                               \
+    if (det) conv_wgrad_smallcb_kernel<CB_, true><<<(unsigned)blocks, 256, smem, st>>>(small, big, part, NB, h, w, Cs, rpb); \
+    else conv_wgrad_smallcb_kernel<CB_, false><<<(unsigned)blocks, 256, smem, st>>>(small, big, dW, NB, h, w, Cs, rpb); \
+  } while (0)
+    if (det)
+      if (int rc = slots_ws(blocks)) return rc;
     switch (Cb) {
-      case 1: conv_wgrad_smallcb_kernel<1><<<(unsigned)blocks, 256, smem, st>>>(small, big, dW, NB, h, w, Cs, rpb); break;
-      case 2: conv_wgrad_smallcb_kernel<2><<<(unsigned)blocks, 256, smem, st>>>(small, big, dW, NB, h, w, Cs, rpb); break;
-      case 3: conv_wgrad_smallcb_kernel<3><<<(unsigned)blocks, 256, smem, st>>>(small, big, dW, NB, h, w, Cs, rpb); break;
-      default: conv_wgrad_smallcb_kernel<4><<<(unsigned)blocks, 256, smem, st>>>(small, big, dW, NB, h, w, Cs, rpb); break;
+      case 1: WGRAD_SMALLCB(1); break;
+      case 2: WGRAD_SMALLCB(2); break;
+      case 3: WGRAD_SMALLCB(3); break;
+      default: WGRAD_SMALLCB(4); break;
     }
+#undef WGRAD_SMALLCB
     RL_CHECK_LAUNCH();
-    return B200RL_OK;
+    return det ? det_sum_slots(part, (int)blocks, nW, dW, nW, nullptr, st) : B200RL_OK;
   }
   const int tcs = ceil_div(Cs, 64), tcb = ceil_div(Cb, 64);
   const int base = tcs * tcb * 16;
   long long splits = max(1LL, min((long long)ceil_div(4 * kNumSMs, base), Mtot / 256));
   long long rps = ((Mtot + splits - 1) / splits + 15) / 16 * 16;
   splits = (Mtot + rps - 1) / rps;
-  conv_wgrad_kernel<<<dim3(tcb, tcs, (unsigned)(16 * splits)), 256, 0, st>>>(small, big, dW, NB, h, w, Cs, Cb, rps);
+  const dim3 grid(tcb, tcs, (unsigned)(16 * splits));
+  if (det) {
+    if (int rc = slots_ws(splits)) return rc;
+    conv_wgrad_kernel<true><<<grid, 256, 0, st>>>(small, big, part, NB, h, w, Cs, Cb, rps);
+    RL_CHECK_LAUNCH();
+    return det_sum_slots(part, (int)splits, nW, dW, nW, nullptr, st);
+  }
+  conv_wgrad_kernel<false><<<grid, 256, 0, st>>>(small, big, dW, NB, h, w, Cs, Cb, rps);
   RL_CHECK_LAUNCH();
   return B200RL_OK;
 }

@@ -121,8 +121,10 @@ conv_up_thin_kernel(const float* __restrict__ small, const float* __restrict__ W
 // CTA tile = up to 32 consecutive small pixels of one image row; the 4 big rows they touch are staged (zero-padded)
 // in shared memory, lane = small channel, each warp walks 4 of the pixels: per pixel 1 LDS + 8*CB broadcast LDS.64
 // feed 16*CB FMAs on register accumulators; one cross-warp + atomic reduction per CTA at the very end.
+// DET: the warps add their accumulators to shared memory one after another in warp order, and the CTA stores its partials
+// to slot blockIdx.x of the slot array dW (Cs*CB*16 floats per slot; det_sum_slots adds the slots).
 // ---------------------------------------------------------------------------------------------------------
-template <int CB>
+template <int CB, bool DET>
 __global__ void __launch_bounds__(256, 2)
 conv_wgrad_thin_kernel(const float* __restrict__ small, const float* __restrict__ big, float* __restrict__ dW, int NB,
                        int h, int w, int Cs, int tiles_per_row) {
@@ -200,16 +202,29 @@ conv_wgrad_thin_kernel(const float* __restrict__ small, const float* __restrict_
       }
     }
     // cross-warp reduction in shared memory, then one atomic per output element and CTA
+    if constexpr (DET) {
+      for (int wv = 0; wv < 8; ++wv) {
+        __syncthreads();
+        if (warp == wv) {
 #pragma unroll
-    for (int ky = 0; ky < 4; ++ky)
+          for (int ky = 0; ky < 4; ++ky)
 #pragma unroll
-      for (int f = 0; f < 4 * CB; ++f) atomicAdd(&Red[(ky * 4 * CB + f) * Cs + g * 32 + lane], acc[ky][f]);
+            for (int f = 0; f < 4 * CB; ++f) Red[(ky * 4 * CB + f) * Cs + g * 32 + lane] += acc[ky][f];
+        }
+      }
+    } else {
+#pragma unroll
+      for (int ky = 0; ky < 4; ++ky)
+#pragma unroll
+        for (int f = 0; f < 4 * CB; ++f) atomicAdd(&Red[(ky * 4 * CB + f) * Cs + g * 32 + lane], acc[ky][f]);
+    }
   }
   __syncthreads();
   for (int e = threadIdx.x; e < 16 * CB * Cs; e += blockDim.x) {
     const int cs = e % Cs, q = e / Cs;                      // q = ky*(4*CB) + kx*CB + cb
     const int ky = q / (4 * CB), rem = q - ky * 4 * CB, kx = rem / CB, cb = rem - kx * CB;
-    atomicAdd(&dW[((long long)cs * CB + cb) * 16 + ky * 4 + kx], Red[e]);
+    if constexpr (DET) dW[(long long)blockIdx.x * Cs * CB * 16 + ((long long)cs * CB + cb) * 16 + ky * 4 + kx] = Red[e];
+    else atomicAdd(&dW[((long long)cs * CB + cb) * 16 + ky * 4 + kx], Red[e]);
   }
 }
 
@@ -420,8 +435,10 @@ conv_up_thin2_kernel(const float* __restrict__ small_, const float* __restrict__
 // small row (blockIdx.y = 32-channel group).  The 4 image rows a small row touches are staged twice, left-padded by 3 and by
 // 5 floats: pixel x's 12-float patch row starts at float 6x (even x, first copy) or 6x+2 (odd x, second copy), both 16-byte
 // aligned LDS.128.  One shared-memory + global atomic flush per CTA.
+// DET: the warps add their accumulators to shared memory one after another in warp order, and the CTA stores its 32
+// channels to slot blockIdx.x of the slot array dW (Cs*3*16 floats per slot; det_sum_slots adds the slots).
 constexpr int WT_ROW = 200;
-template <int NWARPS>
+template <int NWARPS, bool DET>
 __global__ void __launch_bounds__(NWARPS * 32)
 conv_wgrad_thin2_kernel(const float* __restrict__ small_, const float* __restrict__ big, float* __restrict__ dW, int NB, int h,
                         int Cs) {
@@ -483,17 +500,33 @@ conv_wgrad_thin2_kernel(const float* __restrict__ small_, const float* __restric
     }
   }
   // acc[q][c]: patch floats f = 2q, 2q+1 of row kg (k = kg*12 + f), channel csg*4 + c
+  if constexpr (DET) {
+    for (int wv = 0; wv < NWARPS; ++wv) {
+      __syncthreads();
+      if (warp == wv) {
 #pragma unroll
-  for (int q = 0; q < 6; ++q)
+        for (int q = 0; q < 6; ++q)
 #pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      atomicAdd(&Red[(kg * 12 + 2 * q) * 32 + csg * 4 + c], lo32(acc[q][c]));
-      atomicAdd(&Red[(kg * 12 + 2 * q + 1) * 32 + csg * 4 + c], hi32(acc[q][c]));
+          for (int c = 0; c < 4; ++c) {
+            Red[(kg * 12 + 2 * q) * 32 + csg * 4 + c] += lo32(acc[q][c]);
+            Red[(kg * 12 + 2 * q + 1) * 32 + csg * 4 + c] += hi32(acc[q][c]);
+          }
+      }
     }
+  } else {
+#pragma unroll
+    for (int q = 0; q < 6; ++q)
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        atomicAdd(&Red[(kg * 12 + 2 * q) * 32 + csg * 4 + c], lo32(acc[q][c]));
+        atomicAdd(&Red[(kg * 12 + 2 * q + 1) * 32 + csg * 4 + c], hi32(acc[q][c]));
+      }
+  }
   __syncthreads();
   for (int e = threadIdx.x; e < 48 * 32; e += blockDim.x) {
     const int cs = g * 32 + (e & 31), k = e >> 5, tap = k / 3, cb = k - tap * 3;      // k = tap * 3 + cb
-    atomicAdd(&dW[((long long)cs * 3 + cb) * 16 + tap], Red[e]);
+    if constexpr (DET) dW[(long long)blockIdx.x * Cs * 48 + ((long long)cs * 3 + cb) * 16 + tap] = Red[e];
+    else atomicAdd(&dW[((long long)cs * 3 + cb) * 16 + tap], Red[e]);
   }
 }
 
@@ -551,15 +584,32 @@ int b200rl_conv_up_thin(const float* small, const float* W, float* big, const fl
   return B200RL_OK;
 }
 
+// deterministic mode: per-CTA partials in slots of Cs*Cb*16 floats (det_workspace), added to dW in slot order
 int b200rl_conv_wgrad_thin(const float* small, const float* big, float* dW, int NB, int h, int w, int Cs, int Cb,
                            cudaStream_t st) {
+  const bool det = det_mode();
+  const long long nW = (long long)Cs * Cb * 16;
+  float* part = nullptr;
+  auto slots_ws = [&](long long slots) -> int {
+    void* ws = nullptr;
+    if (int rc = det_workspace(sizeof(float) * nW * slots, st, &ws)) return rc;
+    part = static_cast<float*>(ws);
+    return B200RL_OK;
+  };
   if (Cb == 3 && w == 32 && Cs % 32 == 0) {
     constexpr int NW = 4;
     const long long rows = (long long)NB * h;
     long long bx = (rows + NW - 1) / NW;
     const long long cap = (4LL * kNumSMs) / (Cs / 32) > 0 ? (4LL * kNumSMs) / (Cs / 32) : 1;
     if (bx > cap) bx = cap;
-    conv_wgrad_thin2_kernel<NW><<<dim3((unsigned)bx, Cs / 32), NW * 32, 0, st>>>(small, big, dW, NB, h, Cs);
+    const dim3 grid((unsigned)bx, Cs / 32);
+    if (det) {
+      if (int rc = slots_ws(bx)) return rc;
+      conv_wgrad_thin2_kernel<NW, true><<<grid, NW * 32, 0, st>>>(small, big, part, NB, h, Cs);
+      RL_CHECK_LAUNCH();
+      return det_sum_slots(part, (int)bx, nW, dW, nW, nullptr, st);
+    }
+    conv_wgrad_thin2_kernel<NW, false><<<grid, NW * 32, 0, st>>>(small, big, dW, NB, h, Cs);
     RL_CHECK_LAUNCH();
     return B200RL_OK;
   }
@@ -568,12 +618,22 @@ int b200rl_conv_wgrad_thin(const float* small, const float* big, float* dW, int 
   // ~13 KB of smem and 80 registers per thread: 6 CTAs per SM hide the stage -> compute latency of a 32-pixel tile
   long long blocks = ntiles < 6LL * kNumSMs ? ntiles : 6LL * kNumSMs;
   const size_t smem = sizeof(float) * (4 * (2 * 32 + 2) * Cb + 32 * 32 + 16 * Cb * Cs);
+  if (det)
+    if (int rc = slots_ws(blocks)) return rc;
+#define WGRAD_THIN(CB_)                                                                                               \
+  do {                                                                                                                \
+    if (det)                                                                                                          \
+      conv_wgrad_thin_kernel<CB_, true><<<(unsigned)blocks, 256, smem, st>>>(small, big, part, NB, h, w, Cs, tiles_per_row); \
+    else                                                                                                              \
+      conv_wgrad_thin_kernel<CB_, false><<<(unsigned)blocks, 256, smem, st>>>(small, big, dW, NB, h, w, Cs, tiles_per_row); \
+  } while (0)
   switch (Cb) {
-    case 1: conv_wgrad_thin_kernel<1><<<(unsigned)blocks, 256, smem, st>>>(small, big, dW, NB, h, w, Cs, tiles_per_row); break;
-    case 2: conv_wgrad_thin_kernel<2><<<(unsigned)blocks, 256, smem, st>>>(small, big, dW, NB, h, w, Cs, tiles_per_row); break;
-    case 3: conv_wgrad_thin_kernel<3><<<(unsigned)blocks, 256, smem, st>>>(small, big, dW, NB, h, w, Cs, tiles_per_row); break;
-    default: conv_wgrad_thin_kernel<4><<<(unsigned)blocks, 256, smem, st>>>(small, big, dW, NB, h, w, Cs, tiles_per_row); break;
+    case 1: WGRAD_THIN(1); break;
+    case 2: WGRAD_THIN(2); break;
+    case 3: WGRAD_THIN(3); break;
+    default: WGRAD_THIN(4); break;
   }
+#undef WGRAD_THIN
   RL_CHECK_LAUNCH();
-  return B200RL_OK;
+  return det ? det_sum_slots(part, (int)blocks, nW, dW, nW, nullptr, st) : B200RL_OK;
 }

@@ -147,8 +147,9 @@ int launch_cfg(const float* A, const float* B, float* C, const float* bias, int 
                int ldc, int transA, int transB, int accumulate, cudaStream_t st) {
   const int tm = ceil_div(M, BM), tn = ceil_div(N, BN);
   const int tiles = tm * tn;
+  // split-K adds its partial tiles with atomics: deterministic mode runs the whole K in each output tile instead
   int splits = 1;
-  if (tiles < kNumSMs && K >= 8 * BK) {
+  if (tiles < kNumSMs && K >= 8 * BK && !det_mode()) {
     splits = min(ceil_div(2 * kNumSMs, tiles), K / (4 * BK));
     if (splits < 1) splits = 1;
   }

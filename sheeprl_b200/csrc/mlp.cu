@@ -30,8 +30,10 @@ struct BG {
 // tiles with register prefetch of the next k-step (these products are latency- not throughput-bound: without the
 // prefetch every k-step pays a full L2 round trip).  blockIdx.z = net * ksplit + split; with ksplit > 1 each CTA
 // reduces a K-slice and adds its partial tile with fp32 atomics (weight gradients: long K, tiny output).
-template <int BM, int BN, int TM, int TN, int BK>
-__global__ void __launch_bounds__(256) bgemm_kernel(const BG g, const int ksplit, const int kper) {
+// DET: the partial tile (and row sums) of split blockIdx.z go to slot blockIdx.z of `part` ([nets * ksplit][M][N], then
+// [nets * ksplit][M] row sums), and bgemm_splitk_reduce_kernel adds the slots in split order.
+template <int BM, int BN, int TM, int TN, int BK, bool DET>
+__global__ void __launch_bounds__(256) bgemm_kernel(const BG g, const int ksplit, const int kper, float* __restrict__ part) {
   constexpr int NT = (BM / TM) * (BN / TN);
   static_assert(NT == 256, "256 threads");
   constexpr int EA = BM * BK / NT, EB = BN * BK / NT;
@@ -127,6 +129,13 @@ __global__ void __launch_bounds__(256) bgemm_kernel(const BG g, const int ksplit
       const int m = m0 + ty * TM + i;
       if (m >= g.M) continue;
       const int n = n0 + tx * TN;
+      if constexpr (DET) {
+        float* c = part + ((size_t)blockIdx.z * g.M + m) * g.N + n;
+#pragma unroll
+        for (int j = 0; j < TN; ++j)
+          if (n + j < g.N) c[j] = acc[i][j];
+        continue;
+      }
       float* c = C + m * g.ldc + n;
       bool done = false;
       if constexpr (TN == 2) {
@@ -162,7 +171,8 @@ __global__ void __launch_bounds__(256) bgemm_kernel(const BG g, const int ksplit
   }
   if (want_rsum && tid < BM && m0 + tid < g.M) {
     float* r = g.rsum + net * g.strideRsum + m0 + tid;
-    if (ksplit > 1) atomicAdd(r, rs);
+    if (ksplit > 1 && DET) part[(size_t)gridDim.z * g.M * g.N + (size_t)blockIdx.z * g.M + m0 + tid] = rs;
+    else if (ksplit > 1) atomicAdd(r, rs);
     else *r = g.accumulate ? *r + rs : rs;
   }
 }
@@ -176,6 +186,27 @@ __global__ void bgemm_zero_kernel(const BG g) {
     C[(i / g.N) * g.ldc + (i % g.N)] = 0.f;
   if (g.rsum && blockIdx.x == 0)
     for (int m = threadIdx.x; m < g.M; m += blockDim.x) g.rsum[net * g.strideRsum + m] = 0.f;
+}
+
+// C[net] (+)= sum_z part[net * ksplit + z] and rsum[net] likewise, z ascending (deterministic split-K)
+__global__ void bgemm_splitk_reduce_kernel(const BG g, const int ksplit, const float* __restrict__ part) {
+  const int net = blockIdx.z;
+  const long long MN = (long long)g.M * g.N;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < MN) {
+    const float* p = part + (size_t)net * ksplit * MN + i;
+    float s = 0.f;
+    for (int z = 0; z < ksplit; ++z) s += __ldcg(p + (size_t)z * MN);
+    float* c = g.C + net * g.strideC + (i / g.N) * g.ldc + (i % g.N);
+    *c = g.accumulate ? *c + s : s;
+  }
+  if (g.rsum && i < g.M) {
+    const float* p = part + (size_t)gridDim.z * ksplit * MN + (size_t)net * ksplit * g.M + i;
+    float s = 0.f;
+    for (int z = 0; z < ksplit; ++z) s += __ldcg(p + (size_t)z * g.M);
+    float* r = g.rsum + net * g.strideRsum + i;
+    *r = g.accumulate ? *r + s : s;
+  }
 }
 
 }  // namespace
@@ -210,16 +241,30 @@ extern "C" int b200rl_bgemm(const float* A, long long sam, long long sak, long l
   int kper = ((K + ksplit - 1) / ksplit + BK - 1) / BK * BK;
   ksplit = (K + kper - 1) / kper;
   RL_CHECK_ARG((long long)nets * ksplit <= 65535, "too many networks x K-splits for grid.z");
+  dim3 grid(tx, ty, nets * ksplit);
+  if (ksplit > 1 && det_mode()) {
+    void* ws = nullptr;
+    const size_t slots = (size_t)nets * ksplit;
+    if (int rc = det_workspace(sizeof(float) * slots * M * ((size_t)N + 1), st, &ws)) return rc;
+    float* part = static_cast<float*>(ws);
+    if (BMv == 64 && BNv == 64) bgemm_kernel<64, 64, 4, 4, BK, true><<<grid, 256, 0, st>>>(g, ksplit, kper, part);
+    else if (BMv == 64) bgemm_kernel<64, 32, 4, 2, BK, true><<<grid, 256, 0, st>>>(g, ksplit, kper, part);
+    else bgemm_kernel<32, 32, 2, 2, BK, true><<<grid, 256, 0, st>>>(g, ksplit, kper, part);
+    RL_CHECK_LAUNCH();
+    const long long cover = (long long)M * N > M ? (long long)M * N : M;
+    bgemm_splitk_reduce_kernel<<<dim3((unsigned)((cover + 255) / 256), 1, nets), 256, 0, st>>>(g, ksplit, part);
+    RL_CHECK_LAUNCH();
+    return B200RL_OK;
+  }
   if (ksplit > 1 && !accumulate) {
     const long long total = (long long)M * N;
     int zb = (int)((total + 255) / 256);
     if (zb > 64) zb = 64;
     bgemm_zero_kernel<<<dim3(zb, 1, nets), 256, 0, st>>>(g);
   }
-  dim3 grid(tx, ty, nets * ksplit);
-  if (BMv == 64 && BNv == 64) bgemm_kernel<64, 64, 4, 4, BK><<<grid, 256, 0, st>>>(g, ksplit, kper);
-  else if (BMv == 64) bgemm_kernel<64, 32, 4, 2, BK><<<grid, 256, 0, st>>>(g, ksplit, kper);
-  else bgemm_kernel<32, 32, 2, 2, BK><<<grid, 256, 0, st>>>(g, ksplit, kper);
+  if (BMv == 64 && BNv == 64) bgemm_kernel<64, 64, 4, 4, BK, false><<<grid, 256, 0, st>>>(g, ksplit, kper, nullptr);
+  else if (BMv == 64) bgemm_kernel<64, 32, 4, 2, BK, false><<<grid, 256, 0, st>>>(g, ksplit, kper, nullptr);
+  else bgemm_kernel<32, 32, 2, 2, BK, false><<<grid, 256, 0, st>>>(g, ksplit, kper, nullptr);
   RL_CHECK_LAUNCH();
   return B200RL_OK;
 }

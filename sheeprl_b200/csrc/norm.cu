@@ -53,7 +53,9 @@ ln_act_fwd_kernel(const float* __restrict__ X, const float* __restrict__ gamma, 
 }
 
 // CPL = channels per lane held in registers for the dgamma/dbeta partial sums (C <= 32*CPL).
-template <int CPL>
+// DET: dgamma / dbeta are slot arrays with a row stride of 2*C floats, one slot per warp; each warp writes
+// its own partials there (CPL == 0: accumulates them there, row by row) in place of the shared and global atomics.
+template <int CPL, bool DET>
 __global__ void __launch_bounds__(256)
 ln_act_bwd_kernel(const float* __restrict__ X, const float* __restrict__ gamma, const float* __restrict__ beta,
                   const float* dY, float* dX, float* __restrict__ dgamma, float* __restrict__ dbeta,
@@ -69,8 +71,12 @@ ln_act_bwd_kernel(const float* __restrict__ X, const float* __restrict__ gamma, 
   for (int j = 0; j < NACC; ++j) { ag[j] = 0.f; ab[j] = 0.f; }
   const bool want_param = dgamma != nullptr;
   if (CPL == 0 && want_param) {
-    for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) sacc[c] = 0.f;
-    __syncthreads();
+    if constexpr (DET) {
+      for (int c = lane; c < C; c += 32) { dgamma[warp * 2 * C + c] = 0.f; dbeta[warp * 2 * C + c] = 0.f; }
+    } else {
+      for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) sacc[c] = 0.f;
+      __syncthreads();
+    }
   }
   for (long long r = warp; r < M; r += nwarps) {
     const float* x = X + r * ldx;
@@ -106,7 +112,10 @@ ln_act_bwd_kernel(const float* __restrict__ X, const float* __restrict__ gamma, 
       for (int c = lane; c < C; c += 32) {
         float g_, b_;
         body(c, g_, b_);
-        if (want_param) { atomicAdd(&sacc[c], g_); atomicAdd(&sacc[C + c], b_); }
+        if (want_param) {
+          if constexpr (DET) { dgamma[warp * 2 * C + c] += g_; dbeta[warp * 2 * C + c] += b_; }
+          else { atomicAdd(&sacc[c], g_); atomicAdd(&sacc[C + c], b_); }
+        }
       }
     }
     s1 = warp_sum(s1) * invC;
@@ -123,9 +132,12 @@ ln_act_bwd_kernel(const float* __restrict__ X, const float* __restrict__ gamma, 
 #pragma unroll
       for (int j = 0; j < NACC; ++j) {
         const int c = lane + 32 * j;
-        if (c < C) { atomicAdd(&dgamma[c], ag[j]); atomicAdd(&dbeta[c], ab[j]); }
+        if (c < C) {
+          if constexpr (DET) { dgamma[warp * 2 * C + c] = ag[j]; dbeta[warp * 2 * C + c] = ab[j]; }
+          else { atomicAdd(&dgamma[c], ag[j]); atomicAdd(&dbeta[c], ab[j]); }
+        }
       }
-    } else {
+    } else if constexpr (!DET) {
       __syncthreads();
       for (int c = threadIdx.x; c < C; c += blockDim.x) {
         atomicAdd(&dgamma[c], sacc[c]);
@@ -196,6 +208,9 @@ ln_act_fwd_wide_kernel(const float* __restrict__ X, const float* __restrict__ ga
   }
 }
 
+// DET: dgamma / dbeta are slot arrays with a row stride of 2*C floats, one slot per CTA (its threads own disjoint
+// columns): plain stores in place of the global atomics.
+template <bool DET>
 __global__ void __launch_bounds__(WIDE_NT)
 ln_act_bwd_wide_kernel(const float* __restrict__ X, const float* __restrict__ gamma, const float* __restrict__ beta,
                        const float* dY, float* dX, float* __restrict__ dgamma, float* __restrict__ dbeta, long long M, int C,
@@ -266,7 +281,10 @@ ln_act_bwd_wide_kernel(const float* __restrict__ X, const float* __restrict__ ga
 #pragma unroll
     for (int i = 0; i < WNV; ++i) {
       const int c = threadIdx.x + i * WIDE_NT;
-      if (c < n4) {
+      if (c < n4 && DET) {
+        reinterpret_cast<float4*>(dgamma + (long long)blockIdx.x * 2 * C)[c] = ag[i];
+        reinterpret_cast<float4*>(dbeta + (long long)blockIdx.x * 2 * C)[c] = ab[i];
+      } else if (c < n4) {
         atomicAdd(&dgamma[4 * c + 0], ag[i].x); atomicAdd(&dgamma[4 * c + 1], ag[i].y);
         atomicAdd(&dgamma[4 * c + 2], ag[i].z); atomicAdd(&dgamma[4 * c + 3], ag[i].w);
         atomicAdd(&dbeta[4 * c + 0], ab[i].x); atomicAdd(&dbeta[4 * c + 1], ab[i].y);
@@ -285,6 +303,8 @@ bool wide_ok(int C, long long ld0, long long ld1, long long ld2, const void* p0,
 }
 
 // out[c] (+)= sum_m X[m,c]; blockDim = (32, 8); out pre-zeroed by the host wrapper unless accumulating.
+// DET: `out` is the slot array, the CTA's partial goes to out[blockIdx.y * C + c] (det_sum_slots adds the slots).
+template <bool DET>
 __global__ void col_sum_kernel(const float* __restrict__ X, float* __restrict__ out, long long M, int C,
                                long long ldx, long long rows_per_block) {
   __shared__ float red[8][33];
@@ -300,24 +320,45 @@ __global__ void col_sum_kernel(const float* __restrict__ X, float* __restrict__ 
     float t = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) t += red[i][threadIdx.x];
-    atomicAdd(&out[c], t);
+    if constexpr (DET) out[(long long)blockIdx.y * C + c] = t;
+    else atomicAdd(&out[c], t);
   }
 }
 
 // Narrow contiguous matrices (C <= 32, ldx == C: the 3-channel image gradient behind the decoder's output bias): the
 // matrix is read as one flat float4 stream.  The total thread count is a multiple of C, so the column of each of a
 // thread's 4 vector slots never changes across its grid-stride iterations: 4 register accumulators, no per-element modulo.
+// DET: the CTA's 1024 accumulators are staged in shared memory and thread c < C adds those of column c in thread order
+// (then, in CTA 0, the unaligned tail) into slot out[blockIdx.x * C + c]: no shared or global atomics.
+template <bool DET>
 __global__ void __launch_bounds__(256)
 col_sum_narrow_kernel(const float* __restrict__ X, float* __restrict__ out, long long total, int C) {
-  __shared__ float bins[32];
-  if (threadIdx.x < 32) bins[threadIdx.x] = 0.f;
-  __syncthreads();
+  __shared__ float bins[DET ? 1024 : 32];
+  if constexpr (!DET) {
+    if (threadIdx.x < 32) bins[threadIdx.x] = 0.f;
+    __syncthreads();
+  }
   const long long tid = (long long)blockIdx.x * blockDim.x + threadIdx.x, nt = (long long)gridDim.x * blockDim.x;
   const long long n4 = total >> 2;
   float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
   for (long long j = tid; j < n4; j += nt) {
     const float4 v = __ldg(reinterpret_cast<const float4*>(X) + j);
     a0 += v.x; a1 += v.y; a2 += v.z; a3 += v.w;
+  }
+  if constexpr (DET) {
+    float* b = bins + 4 * threadIdx.x;
+    b[0] = a0; b[1] = a1; b[2] = a2; b[3] = a3;
+    __syncthreads();
+    if (threadIdx.x < C) {
+      const int c = threadIdx.x;
+      const long long base = 4LL * blockIdx.x * blockDim.x;      // flat element index of bins[0]
+      float s = 0.f;
+      for (int p = (int)((c - base % C + C) % C); p < 4 * (int)blockDim.x; p += C) s += bins[p];
+      if (blockIdx.x == 0)
+        for (long long i = (n4 << 2) + (c - (n4 << 2) % C + C) % C; i < total; i += C) s += X[i];
+      out[(long long)blockIdx.x * C + c] = s;
+    }
+    return;
   }
   const int c0 = (int)((4 * tid) % C);
   if (tid < n4) {
@@ -393,18 +434,20 @@ ln_act_fwd_vec_kernel(const float* __restrict__ X, const float* __restrict__ gam
   }
 }
 
-template <int LPR, int NV>
+// DET: dgamma / dbeta are slot arrays with a row stride of 2*C floats, one slot per warp: the warp's row groups are
+// added by a fixed butterfly and lanes 0..LPR-1 store the sums, in place of the shared and global atomics.
+template <int LPR, int NV, bool DET>
 __global__ void __launch_bounds__(256)
 ln_act_bwd_vec_kernel(const float* __restrict__ X, const float* __restrict__ gamma, const float* __restrict__ beta,
                       const float* dY, float* dX, float* __restrict__ dgamma, float* __restrict__ dbeta, long long M,
                       long long ldx, long long lddy, long long lddx, float eps, int act) {
   constexpr int RPW = 32 / LPR, C = 4 * LPR * NV;
-  __shared__ float sacc[2 * C];
+  __shared__ float sacc[DET ? 1 : 2 * C];
   const int lane = threadIdx.x & 31, lr = lane % LPR, sub = lane / LPR;
   const long long gwarp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
   const bool want_param = dgamma != nullptr;
-  if (want_param) {
+  if (want_param && !DET) {
     for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) sacc[c] = 0.f;
     __syncthreads();
   }
@@ -465,7 +508,22 @@ ln_act_bwd_vec_kernel(const float* __restrict__ X, const float* __restrict__ gam
       }
     }
   }
-  if (want_param) {
+  if (want_param && DET) {
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+#pragma unroll
+      for (int o = LPR; o < 32; o <<= 1) {
+        ag[i].x += __shfl_xor_sync(0xffffffffu, ag[i].x, o); ag[i].y += __shfl_xor_sync(0xffffffffu, ag[i].y, o);
+        ag[i].z += __shfl_xor_sync(0xffffffffu, ag[i].z, o); ag[i].w += __shfl_xor_sync(0xffffffffu, ag[i].w, o);
+        ab[i].x += __shfl_xor_sync(0xffffffffu, ab[i].x, o); ab[i].y += __shfl_xor_sync(0xffffffffu, ab[i].y, o);
+        ab[i].z += __shfl_xor_sync(0xffffffffu, ab[i].z, o); ab[i].w += __shfl_xor_sync(0xffffffffu, ab[i].w, o);
+      }
+      if (sub == 0) {
+        reinterpret_cast<float4*>(dgamma + gwarp * 2 * C)[lr + i * LPR] = ag[i];
+        reinterpret_cast<float4*>(dbeta + gwarp * 2 * C)[lr + i * LPR] = ab[i];
+      }
+    }
+  } else if (want_param) {
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
       const int c = 4 * (lr + i * LPR);
@@ -575,13 +633,41 @@ extern "C" int b200rl_ln_act_bwd(const float* X, const float* gamma, const float
     RL_CUDA(cudaMemsetAsync(dbeta, 0, sizeof(float) * C, st));
   }
   if (M <= 0) return B200RL_OK;
+  // deterministic mode: the kernels write per-warp (per-CTA on the wide route) partials to `slots` slots of 2*C floats
+  // and det_sum_slots adds them to dgamma / dbeta in slot order
+  const bool det = dgamma && det_mode();
+  float* pg = dgamma;
+  float* pb = dbeta;
+  auto slots_ws = [&](long long slots) -> int {
+    void* ws = nullptr;
+    if (int rc = det_workspace(sizeof(float) * 2 * (size_t)C * slots, st, &ws)) return rc;
+    pg = static_cast<float*>(ws);
+    pb = pg + C;
+    return B200RL_OK;
+  };
+  auto finish = [&](long long slots) -> int {
+    RL_CHECK_LAUNCH();
+    if (!det) return B200RL_OK;
+    return det_sum_slots(pg, (int)slots, 2LL * C, dgamma, C, dbeta, st);
+  };
   if (route == ROUTE_VEC) {
     // every CTA ends with 2*C global atomics into dgamma / dbeta: for wide rows (a warp already keeps >= 2 KB in flight) two
-    // CTAs per SM saturate HBM and cut that traffic 4x (ncu: [16384,512] ran at 0.34 of the HBM peak with 1184 CTAs)
-    const int bwd_cap = (dgamma && C >= 256) ? 2 * kNumSMs : (1 << 30);
+    // CTAs per SM saturate HBM and cut that traffic 4x (ncu: [16384,512] ran at 0.34 of the HBM peak with 1184 CTAs).
+    // Deterministic mode takes the same cap at every width: it bounds the slots the reduction reads.
+    const int bwd_cap = (dgamma && (C >= 256 || det)) ? 2 * kNumSMs : (1 << 30);
+    int vgrid = 0;
 #define LN_BWD_VEC(LPR_, NV_)                                                                                         \
-  ln_act_bwd_vec_kernel<LPR_, NV_><<<min(vec_grid(M, 32 / LPR_), bwd_cap), 256, 0, st>>>(X, gamma, beta, dY, dX, dgamma, \
-                                                                                       dbeta, M, ldx, lddy, lddx, eps, act)
+  do {                                                                                                                \
+    vgrid = min(vec_grid(M, 32 / LPR_), bwd_cap);                                                                     \
+    if (!det) {                                                                                                       \
+      ln_act_bwd_vec_kernel<LPR_, NV_, false><<<vgrid, 256, 0, st>>>(X, gamma, beta, dY, dX, dgamma, dbeta, M, ldx,   \
+                                                                     lddy, lddx, eps, act);                           \
+    } else {                                                                                                          \
+      if (int rc = slots_ws(8LL * vgrid)) return rc;                                                                  \
+      ln_act_bwd_vec_kernel<LPR_, NV_, true><<<vgrid, 256, 0, st>>>(X, gamma, beta, dY, dX, pg, pb, M, ldx, lddy, lddx,\
+                                                                    eps, act);                                        \
+    }                                                                                                                 \
+  } while (0)
     switch (C) {
       case 32: LN_BWD_VEC(8, 1); break;
       case 64: LN_BWD_VEC(16, 1); break;
@@ -598,20 +684,36 @@ extern "C" int b200rl_ln_act_bwd(const float* X, const float* gamma, const float
       default: LN_BWD_VEC(32, 12); break;
     }
 #undef LN_BWD_VEC
-    RL_CHECK_LAUNCH();
-    return B200RL_OK;
+    return finish(8LL * vgrid);
   }
   if (route == ROUTE_WIDE) {
     const int wgrid = (int)(M < 2LL * kNumSMs ? M : 2LL * kNumSMs);
-    ln_act_bwd_wide_kernel<<<wgrid, WIDE_NT, 0, st>>>(X, gamma, beta, dY, dX, dgamma, dbeta, M, C, ldx, lddy, lddx, eps, act);
-    RL_CHECK_LAUNCH();
-    return B200RL_OK;
+    if (det) {
+      if (int rc = slots_ws(wgrid)) return rc;
+      ln_act_bwd_wide_kernel<true><<<wgrid, WIDE_NT, 0, st>>>(X, gamma, beta, dY, dX, pg, pb, M, C, ldx, lddy, lddx, eps,
+                                                              act);
+    } else {
+      ln_act_bwd_wide_kernel<false><<<wgrid, WIDE_NT, 0, st>>>(X, gamma, beta, dY, dX, dgamma, dbeta, M, C, ldx, lddy,
+                                                               lddx, eps, act);
+    }
+    return finish(wgrid);
   }
   int grid = grid_for_rows(M);
   if (dgamma && grid > 2 * kNumSMs) grid = 2 * kNumSMs;  // fewer, longer-lived warps -> fewer flush atomics
-#define LN_BWD(CPL_, SMEM_)                                                                                    \
-  ln_act_bwd_kernel<CPL_><<<grid, 256, SMEM_, st>>>(X, gamma, beta, dY, dX, dgamma, dbeta, M, C, ldx, lddy, lddx, \
-                                                    eps, act)
+  // deterministic mode, C > 512: a slot of 2*C floats per warp, so fewer warps (the route no engine width takes)
+  if (det && C > 512 && grid > 32) grid = 32;
+  if (det)
+    if (int rc = slots_ws(8LL * grid)) return rc;
+  // the default instances are instantiated first: that keeps their code the default path's code before DET
+#define LN_BWD(CPL_, SMEM_)                                                                                           \
+  do {                                                                                                                \
+    if (!det)                                                                                                         \
+      ln_act_bwd_kernel<CPL_, false><<<grid, 256, SMEM_, st>>>(X, gamma, beta, dY, dX, dgamma, dbeta, M, C, ldx, lddy,\
+                                                               lddx, eps, act);                                       \
+    else                                                                                                              \
+      ln_act_bwd_kernel<CPL_, true><<<grid, 256, 0, st>>>(X, gamma, beta, dY, dX, pg, pb, M, C, ldx, lddy, lddx, eps, \
+                                                          act);                                                       \
+  } while (0)
   if (C <= 32) LN_BWD(1, 0);
   else if (C <= 64) LN_BWD(2, 0);
   else if (C <= 128) LN_BWD(4, 0);
@@ -621,13 +723,12 @@ extern "C" int b200rl_ln_act_bwd(const float* X, const float* gamma, const float
     // wide rows (XL: the GRU's joint LayerNorm spans 3*4096 channels): per-CTA gamma/beta partials in opted-in smem
     // (C <= 28000, checked above)
     const size_t smem = sizeof(float) * 2 * (size_t)C;
-    if (smem > 48 * 1024)
-      RL_CUDA(cudaFuncSetAttribute(ln_act_bwd_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (smem > 48 * 1024 && !det)
+      RL_CUDA(cudaFuncSetAttribute(ln_act_bwd_kernel<0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     LN_BWD(0, smem);
   }
 #undef LN_BWD
-  RL_CHECK_LAUNCH();
-  return B200RL_OK;
+  return finish(8LL * grid);
 }
 
 extern "C" int b200rl_col_sum(const float* X, float* out, long long M, int C, long long ldx, int accumulate,
@@ -636,10 +737,18 @@ extern "C" int b200rl_col_sum(const float* X, float* out, long long M, int C, lo
   RL_CHECK_ARG(C > 0 && ldx >= C, "bad C / ld");
   if (!accumulate) RL_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * C, st));
   if (M <= 0) return B200RL_OK;
+  const bool det = det_mode();
+  void* ws = nullptr;
   if (C <= 32 && ldx == C && M * C >= (1 << 16) && (reinterpret_cast<uintptr_t>(X) & 15) == 0) {
     int blocks = 4 * kNumSMs;
     blocks = (blocks + C - 1) / C * C;             // thread count divisible by C: fixed column per vector slot
-    col_sum_narrow_kernel<<<blocks, 256, 0, st>>>(X, out, M * C, C);
+    if (det) {
+      if (int rc = det_workspace(sizeof(float) * blocks * C, st, &ws)) return rc;
+      col_sum_narrow_kernel<true><<<blocks, 256, 0, st>>>(X, static_cast<float*>(ws), M * C, C);
+      RL_CHECK_LAUNCH();
+      return det_sum_slots(static_cast<const float*>(ws), blocks, C, out, C, nullptr, st);
+    }
+    col_sum_narrow_kernel<false><<<blocks, 256, 0, st>>>(X, out, M * C, C);
     RL_CHECK_LAUNCH();
     return B200RL_OK;
   }
@@ -648,7 +757,14 @@ extern "C" int b200rl_col_sum(const float* X, float* out, long long M, int C, lo
   long long rows_per_block = (M + rb - 1) / rb;
   if (rows_per_block < 64) rows_per_block = 64;
   rb = (M + rows_per_block - 1) / rows_per_block;
-  col_sum_kernel<<<dim3(cb, (unsigned)rb), dim3(32, 8), 0, st>>>(X, out, M, C, ldx, rows_per_block);
+  if (det) {
+    if (int rc = det_workspace(sizeof(float) * rb * C, st, &ws)) return rc;
+    col_sum_kernel<true><<<dim3(cb, (unsigned)rb), dim3(32, 8), 0, st>>>(X, static_cast<float*>(ws), M, C, ldx,
+                                                                         rows_per_block);
+    RL_CHECK_LAUNCH();
+    return det_sum_slots(static_cast<const float*>(ws), (int)rb, C, out, C, nullptr, st);
+  }
+  col_sum_kernel<false><<<dim3(cb, (unsigned)rb), dim3(32, 8), 0, st>>>(X, out, M, C, ldx, rows_per_block);
   RL_CHECK_LAUNCH();
   return B200RL_OK;
 }

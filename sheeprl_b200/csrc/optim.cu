@@ -10,6 +10,9 @@
 
 namespace {
 
+// DET: the CTA's partial goes to slot blockIdx.x of `out` (det_sum_slots_d adds the slots in order) in place of a double
+// atomic into out[0].
+template <bool DET>
 __global__ void __launch_bounds__(256)
 sumsq_kernel(const float* __restrict__ x, long long n, double* __restrict__ out) {
   __shared__ double red[8];
@@ -29,7 +32,10 @@ sumsq_kernel(const float* __restrict__ x, long long n, double* __restrict__ out)
   if (threadIdx.x < 32) {
     double r = (threadIdx.x < 8) ? red[threadIdx.x] : 0.0;
     r = warp_sum_d(r);
-    if (threadIdx.x == 0) atomicAdd(out, r);
+    if (threadIdx.x == 0) {
+      if constexpr (DET) out[blockIdx.x] = r;
+      else atomicAdd(out, r);
+    }
   }
 }
 
@@ -302,7 +308,15 @@ extern "C" int b200rl_sumsq(const float* x, long long n, double* out, cudaStream
   RL_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 15) == 0, "x must be 16-byte aligned");
   RL_CUDA(cudaMemsetAsync(out, 0, sizeof(double), st));
   if (n <= 0) return B200RL_OK;
-  sumsq_kernel<<<stream_grid(n / 4 + 1), 256, 0, st>>>(x, n, out);
+  const int grid = stream_grid(n / 4 + 1);
+  if (det_mode()) {
+    void* ws = nullptr;
+    if (int rc = det_workspace(sizeof(double) * grid, st, &ws)) return rc;
+    sumsq_kernel<true><<<grid, 256, 0, st>>>(x, n, static_cast<double*>(ws));
+    RL_CHECK_LAUNCH();
+    return det_sum_slots_d(static_cast<const double*>(ws), grid, out, st);
+  }
+  sumsq_kernel<false><<<grid, 256, 0, st>>>(x, n, out);
   RL_CHECK_LAUNCH();
   return B200RL_OK;
 }

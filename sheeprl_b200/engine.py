@@ -27,6 +27,7 @@ from typing import Dict, Mapping, Optional, Sequence
 import torch
 
 from sheeprl_b200.params import FlatGroup
+from sheeprl_b200.lib import sync_deterministic
 
 ACT_NONE, ACT_SILU = 0, 1
 TWOHOT_LOW, TWOHOT_HIGH = -20.0, 20.0
@@ -534,10 +535,11 @@ class DV3Engine:
 
     def graph_key(self) -> tuple:
         """what a captured step bakes in besides the batch shapes: the learning rates and weight decays (kernel arguments
-        by value)"""
+        by value), the matmul precision and the deterministic mode (which kernels run)"""
         prec = self.ops.matmul_precision() if hasattr(self.ops, "matmul_precision") else "highest"
         return tuple((float(g.optimizer.lr), g.adam_kwargs().get("weight_decay", 0.0))
-                     if getattr(g, "optimizer", None) is not None else -1.0 for g in self.optimizer_groups()) + (prec,)
+                     if getattr(g, "optimizer", None) is not None else -1.0 for g in self.optimizer_groups()) + (
+                         prec, "deterministic" if torch.are_deterministic_algorithms_enabled() else "default")
 
     def step_graph(self):
         if self._graph is None:
@@ -580,6 +582,7 @@ class DV3Engine:
         """data: the reference's batch dict ([T,B,...]; image key uint8 or float 0..255).
         noise: optional injected Exp(1) noise {"post":[T,B,S,D], "img_state":[H,N,S,D],
         "img_action":[list per head of [H+1,N,A_h]]} (parity mode); None -> on-device Philox."""
+        sync_deterministic(self.ops)
         self._draw_noise(noise)
         self._world_model_phase(data)
         # ---- behaviour learning with the updated world model

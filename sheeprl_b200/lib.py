@@ -107,6 +107,18 @@ def declared_symbols() -> Sequence[str]:
     return sorted(_FUNCTIONS)
 
 
+def sync_deterministic(ops) -> bool:
+    """Puts `ops` in deterministic mode when torch.are_deterministic_algorithms_enabled(), the process-wide switch the
+    reference's CLI sets from `torch_use_deterministic_algorithms` (configs/config.yaml), and out of it otherwise.
+    Every engine train() and player call starts with it, so a run that flips torch's switch between calls follows it.
+    Backends without the setter (the CPU test doubles) are left alone.  Returns the mode."""
+    on = torch.are_deterministic_algorithms_enabled()
+    setter = getattr(ops, "set_deterministic", None)
+    if setter is not None:
+        setter(on)
+    return on
+
+
 def _p(t: Optional[torch.Tensor]):
     return None if t is None else t.data_ptr()
 
@@ -180,6 +192,14 @@ class CudaOps:
 
     def matmul_precision(self) -> str:
         return "highest" if self.lib.b200rl_get_matmul_precision() == 3 else "high"
+
+    def set_deterministic(self, on: bool) -> None:
+        """Deterministic mode of the library (process-wide): every float reduction in a fixed order, so that the same
+        inputs give bit-identical outputs on the same GPU type.  Engines follow torch's switch (`sync_deterministic`)."""
+        self._ck(self.lib.b200rl_set_deterministic(int(bool(on))), 0)
+
+    def deterministic(self) -> bool:
+        return bool(self.lib.b200rl_get_deterministic())
 
     def gemm(self, A, B, C, transA: bool, transB: bool, bias=None, accumulate: bool = False):
         _f32(A, B, C, bias)
