@@ -187,6 +187,20 @@ int b200rl_head_sample_supported(const float* X, const float* W, int Kin, int A,
 int b200rl_head_sample(const float* X, const float* W, const float* bias, const float* noise, float* raw, float* onehot,
                        long long M, int Kin, int A, long long ldx, long long ldw, long long ldr, long long ldn,
                        long long ldo, float unimix, cudaStream_t stream);
+/* MinedojoActor's masked, chained sample (sheeprl/algos/dreamer_v3/agent.py:898-932) in one launch: the three heads
+ * [K0 | K1 | K2] are consecutive column blocks of each row of raw, noise and onehot.  Per row: head 0 with
+ * mask_action_type; head 1 with mask_craft_smelt when head 0 drew class 15 (craft), else unmasked; head 2 with
+ * mask_equip_place after 16 / 17 (equip / place), mask_destroy after 18 (destroy), else unmasked.  Masks are float
+ * rows (nonzero = allowed; NULL = all allowed) applied after unimix; the draw is b200rl_cat_sample's, so with every class
+ * allowed the one-hot rows are bit-identical to three b200rl_cat_sample calls.  A mask row that allows no class leaves
+ * its head unmasked (the reference's distribution would have NaN logits).  Only the K0 + K1 + K2 one-hot columns of a
+ * row are written.  `_supported`: every head has 1 to 2048 classes. */
+int b200rl_minedojo_sample_supported(int K0, int K1, int K2);
+int b200rl_minedojo_sample(const float* raw, const float* noise, float* onehot, const float* mask_action_type,
+                           const float* mask_craft_smelt, const float* mask_equip_place, const float* mask_destroy,
+                           long long M, int K0, int K1, int K2, long long ldr, long long ldn, long long ldo,
+                           long long ld_action_type, long long ld_craft_smelt, long long ld_equip_place,
+                           long long ld_destroy, float unimix, cudaStream_t stream);
 int b200rl_cat_sample_bwd(const float* raw, const float* dz, const float* dmix, float* draw, long long M, int groups,
                           int classes, long long ldr, long long lddz, long long lddm, long long lddr, float unimix,
                           cudaStream_t stream);

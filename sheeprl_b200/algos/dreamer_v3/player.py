@@ -99,8 +99,11 @@ class PlayerDV3:
         """obs[key]: `[1, num_envs, C, H, W]` — float32 already normalised as the reference's `prepare_obs` passes it
         (dreamer_v3/utils.py:80-91), or raw uint8 (normalised by the kernel: 4x less host->device traffic).
         `noise` (extra, optional): {"z": Exp(1) [E, S*D], "a": Exp(1) / N(0,1) [E, A]} for parity tests.
-        `mask` is ignored, as the reference's `Actor.forward` ignores it (the reference's `test()` passes the observation's
-        `mask*` keys, an empty dict for environments without them)."""
+        `mask`: the observation's `mask_*` keys.  The plain actor ignores it, as the reference's `Actor.forward` does.
+        The MineDojo actor (algo.actor.cls MinedojoActor) applies them after unimix, chained on the functional action
+        (agent.py:898-932), in one kernel after the head products; a non-empty dict must hold all four keys.  An empty
+        dict or None acts unmasked (the reference's `test()` passes {} for environments without mask keys, which its
+        MinedojoActor cannot take)."""
         e, ops, E = self.eng, self.eng.ops, self.num_envs
         sync_deterministic(ops)
         Z = e.Z
@@ -152,6 +155,14 @@ class PlayerDV3:
             ops.cont_action_fwd(raw, na, self.actions[0], None, float(ac.min_std), float(ac.max_std), float(ac.init_std),
                                 float(ac.action_clip))
             return (self.actions.clone(),)
+        if e.minedojo and mask:
+            ops.minedojo_sample(raw, None if greedy else na, e.unimix, e.actions_dim, self.actions[0],
+                                *self._mask_rows(mask))
+            out, off = [], 0
+            for ad in e.actions_dim:
+                out.append(self.actions[:, :, off:off + ad].clone())
+                off += ad
+            return tuple(out)
         out, off = [], 0
         for ad in e.actions_dim:
             ops.cat_sample(raw[:, off:off + ad], None if greedy else na[:, off:off + ad], e.unimix, 1, ad,
@@ -159,5 +170,18 @@ class PlayerDV3:
             out.append(self.actions[:, :, off:off + ad].clone())
             off += ad
         return tuple(out)
+
+    def _mask_rows(self, mask) -> Sequence[torch.Tensor]:
+        """the four MineDojo masks as float [num_envs, K] rows on the device (nonzero = allowed), in the kernel's order;
+        a mask with one row applies to every environment"""
+        E, (K0, K1, K2) = self.num_envs, self.actions_dim
+        rows = []
+        for key, k in (("mask_action_type", K0), ("mask_craft_smelt", K1), ("mask_equip_place", K2), ("mask_destroy", K2)):
+            m = torch.as_tensor(mask[key])                 # KeyError for a missing key, as MinedojoActor.forward
+            if m.shape[-1] != k or m.numel() not in (k, E * k):
+                raise ValueError(f"{key}: expected {k} classes for {E} environments, got shape {tuple(m.shape)}")
+            m = m.to(device=self.device, dtype=torch.float32).reshape(-1, k)
+            rows.append(m.expand(E, k).contiguous() if m.shape[0] != E else m.contiguous())
+        return rows
 
     __call__ = get_actions

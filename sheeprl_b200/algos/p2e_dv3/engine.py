@@ -153,11 +153,14 @@ class P2EDV3Engine(DV3Engine):
             self._draw_noise(None)                                                   # post / task rollout streams 0-2
             ops.fill_exponential(self.noise_img_state_expl.view(-1), self.rng_seed, 3, self.rng_t)
             fill = ops.fill_normal if self.is_continuous else ops.fill_exponential
-            fill(self.noise_img_action_expl.view(-1), self.rng_seed, 4, self.rng_t)
+            if not self.minedojo:                                     # the MineDojo actors imagine mode actions
+                fill(self.noise_img_action_expl.view(-1), self.rng_seed, 4, self.rng_t)
         else:
-            self._draw_noise({"post": noise["post"], "img_state": noise["img_state_task"], "img_action": noise["img_action_task"]})
+            self._draw_noise({"post": noise["post"], "img_state": noise["img_state_task"],
+                              "img_action": noise.get("img_action_task")})
             self.noise_img_state_expl.copy_(noise["img_state_expl"].reshape(H, N, Z))
-            self.noise_img_action_expl.copy_(torch.cat([x for x in noise["img_action_expl"]], -1))
+            if not self.minedojo:
+                self.noise_img_action_expl.copy_(torch.cat([x for x in noise["img_action_expl"]], -1))
         self._world_model_phase(data, heads_detached=True)
         self._ensemble_learning(data)
         # the exploration rollout and its losses (the continuous backward re-reads the action noise) use their own noise;

@@ -252,6 +252,110 @@ head_sample_kernel(const float* __restrict__ X, const float* __restrict__ W, con
   cat_sample_lane(mine, on, A, lane, unimix, noise ? noise + m * ldn : nullptr, onehot + m * ldo, nullptr);
 }
 
+// MineDojo functional actions whose argument head is masked (sheeprl/envs/minedojo.py ACTION_MAP; agent.py:905-924)
+constexpr int kMinedojoCraft = 15, kMinedojoEquip = 16, kMinedojoPlace = 17, kMinedojoDestroy = 18;
+
+// One K-way head of one row on one warp, with an optional class mask (nonzero = allowed): unimix over ALL K classes,
+// then the disallowed log-probs become -inf (they are skipped), then torch's Categorical normalisation and the
+// exponential race of cat_sample_kernel (noise == nullptr: the mode).  The loops, expressions and butterfly
+// reductions are cat_sample_kernel's, so with every class allowed the one-hot is bit-identical to it (and to
+// cat_sample_small_kernel, which is bit-identical to it).  A mask that allows no class is ignored: the head falls back
+// to its unmasked distribution.  Returns the drawn class on every lane.
+__device__ __forceinline__ int masked_head_sample(const float* __restrict__ x, int K, const float* __restrict__ mask,
+                                                  const float* __restrict__ noise, float* __restrict__ onehot,
+                                                  float unimix, int lane) {
+  bool any = false;
+  if (mask) {
+    for (int c = lane; c < K; c += 32) any = any || mask[c] != 0.f;
+    any = __any_sync(0xffffffffu, any);
+  }
+  const float* mk = any ? mask : nullptr;
+  float mx = -INFINITY;
+  for (int c = lane; c < K; c += 32) mx = fmaxf(mx, x[c]);
+  mx = warp_max(mx);
+  float sm = 0.f;
+  for (int c = lane; c < K; c += 32) sm += expf(x[c] - mx);
+  sm = warp_sum(sm);
+  const float invK = 1.f / (float)K;
+  float lmx = -INFINITY;
+  for (int c = lane; c < K; c += 32) {
+    if (mk && mk[c] == 0.f) continue;
+    float l = x[c];
+    if (unimix > 0.f) { float pm; l = unimix_logprob(expf(x[c] - mx) / sm, unimix, invK, pm); }
+    lmx = fmaxf(lmx, l);
+  }
+  lmx = warp_max(lmx);
+  float ls = 0.f;
+  for (int c = lane; c < K; c += 32) {
+    if (mk && mk[c] == 0.f) continue;
+    float l = x[c];
+    if (unimix > 0.f) { float pm; l = unimix_logprob(expf(x[c] - mx) / sm, unimix, invK, pm); }
+    ls += expf(l - lmx);
+  }
+  ls = warp_sum(ls);
+  const float lse = lmx + logf(ls);
+  float lgmax = -INFINITY;
+  for (int c = lane; c < K; c += 32) {
+    if (mk && mk[c] == 0.f) continue;
+    float l = x[c];
+    if (unimix > 0.f) { float pm; l = unimix_logprob(expf(x[c] - mx) / sm, unimix, invK, pm); }
+    lgmax = fmaxf(lgmax, l - lse);
+  }
+  lgmax = warp_max(lgmax);
+  float psum = 0.f;
+  for (int c = lane; c < K; c += 32) {
+    if (mk && mk[c] == 0.f) continue;
+    float l = x[c];
+    if (unimix > 0.f) { float pm; l = unimix_logprob(expf(x[c] - mx) / sm, unimix, invK, pm); }
+    psum += expf(l - lse - lgmax);
+  }
+  psum = warp_sum(psum);
+  float best = -INFINITY;
+  int besti = 0x7fffffff;
+  for (int c = lane; c < K; c += 32) {
+    if (mk && mk[c] == 0.f) continue;
+    float l = x[c];
+    if (unimix > 0.f) { float pm; l = unimix_logprob(expf(x[c] - mx) / sm, unimix, invK, pm); }
+    float p = expf(l - lse - lgmax) / psum;
+    if (noise) p = p / noise[c];
+    if (p > best) { best = p; besti = c; }  // strict > keeps the first maximum within a lane
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, besti, o);
+    if (ob > best || (ob == best && oi < besti)) { best = ob; besti = oi; }
+  }
+  for (int c = lane; c < K; c += 32) onehot[c] = (c == besti) ? 1.f : 0.f;
+  return besti;
+}
+
+// MinedojoActor.forward with action masks (agent.py:898-932): one warp per row draws the functional action (head 0,
+// masked by mask_action_type), then the craft / smelt item (head 1, masked by mask_craft_smelt where head 0 drew
+// craft) and the item (head 2, masked by mask_equip_place after equip / place, by mask_destroy after destroy).  The
+// three heads are consecutive column blocks of one row in raw, noise and onehot.  No atomics: every row's result
+// depends on its own inputs only.
+__global__ void __launch_bounds__(256)
+minedojo_sample_kernel(const float* __restrict__ raw, const float* __restrict__ noise, float* __restrict__ onehot,
+                       const float* __restrict__ m_type, const float* __restrict__ m_craft,
+                       const float* __restrict__ m_equip, const float* __restrict__ m_destroy, long long M, int K0,
+                       int K1, int K2, long long ldr, long long ldn, long long ldo, long long ld_type,
+                       long long ld_craft, long long ld_equip, long long ld_destroy, float unimix) {
+  const int lane = threadIdx.x & 31;
+  const long long m = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (m >= M) return;
+  const float* x = raw + m * ldr;
+  const float* q = noise ? noise + m * ldn : nullptr;
+  float* o = onehot + m * ldo;
+  const int a0 = masked_head_sample(x, K0, m_type ? m_type + m * ld_type : nullptr, q, o, unimix, lane);
+  const float* mk1 = (a0 == kMinedojoCraft && m_craft) ? m_craft + m * ld_craft : nullptr;
+  masked_head_sample(x + K0, K1, mk1, q ? q + K0 : nullptr, o + K0, unimix, lane);
+  const float* mk2 = nullptr;
+  if ((a0 == kMinedojoEquip || a0 == kMinedojoPlace) && m_equip) mk2 = m_equip + m * ld_equip;
+  else if (a0 == kMinedojoDestroy && m_destroy) mk2 = m_destroy + m * ld_destroy;
+  masked_head_sample(x + K0 + K1, K2, mk2, q ? q + K0 + K1 : nullptr, o + K0 + K1, unimix, lane);
+}
+
 __global__ void __launch_bounds__(256)
 cat_sample_bwd_kernel(const float* __restrict__ raw, const float* __restrict__ dz, const float* __restrict__ dmix,
                       float* __restrict__ draw, long long M, int groups, int K, long long ldr, long long lddz,
@@ -512,6 +616,25 @@ extern "C" int b200rl_head_sample(const float* X, const float* W, const float* b
   if (M <= 0) return B200RL_OK;
   head_sample_kernel<<<ceil_div(M * 32, 256), 256, 0, st>>>(X, W, bias, noise, raw, onehot, M, Kin, A, ldx, ldw, ldr, ldn, ldo,
                                                             unimix);
+  RL_CHECK_LAUNCH();
+  return B200RL_OK;
+}
+
+extern "C" int b200rl_minedojo_sample_supported(int K0, int K1, int K2) {
+  return K0 > 0 && K0 <= 2048 && K1 > 0 && K1 <= 2048 && K2 > 0 && K2 <= 2048;
+}
+
+extern "C" int b200rl_minedojo_sample(const float* raw, const float* noise, float* onehot, const float* mask_action_type,
+                                      const float* mask_craft_smelt, const float* mask_equip_place,
+                                      const float* mask_destroy, long long M, int K0, int K1, int K2, long long ldr,
+                                      long long ldn, long long ldo, long long ld_action_type, long long ld_craft_smelt,
+                                      long long ld_equip_place, long long ld_destroy, float unimix, cudaStream_t st) {
+  RL_CHECK_ARG(raw && onehot, "null pointer");
+  RL_CHECK_ARG(b200rl_minedojo_sample_supported(K0, K1, K2), "minedojo_sample: every head has 1 to 2048 classes");
+  if (M <= 0) return B200RL_OK;
+  minedojo_sample_kernel<<<ceil_div(M * 32, 256), 256, 0, st>>>(
+      raw, noise, onehot, mask_action_type, mask_craft_smelt, mask_equip_place, mask_destroy, M, K0, K1, K2, ldr, ldn, ldo,
+      ld_action_type, ld_craft_smelt, ld_equip_place, ld_destroy, unimix);
   RL_CHECK_LAUNCH();
   return B200RL_OK;
 }

@@ -281,8 +281,14 @@ class DV3Engine:
             raise ValueError("There must be at least one encoder, both cnn and mlp encoders are None")     # models.py:420-421
         check_decoder_keys(cfg)
         actor_cls = str(a.actor.get("cls", "Actor"))
-        if actor_cls.endswith("MinedojoActor"):
-            raise NotImplementedError(f"algo.actor.cls = {actor_cls}: the action masks of the MineDojo actor are not built")
+        # MinedojoActor (agent.py:848-932): the Actor's parameters; imagination takes the mode of each head and the
+        # player applies the observation's action masks (PlayerDV3.get_actions)
+        self.minedojo = actor_cls.endswith("MinedojoActor")
+        if self.minedojo and (is_continuous or len(actions_dim) != 3 or int(actions_dim[0]) != 19):
+            raise NotImplementedError(
+                f"algo.actor.cls = {actor_cls}: the MineDojo actor is built for the MineDojo action space only (discrete, "
+                f"three heads, 19 functional actions first), got actions_dim={tuple(actions_dim)}"
+                f"{' continuous' if is_continuous else ''}")
         self.cnn_keys = list(a.cnn_keys.encoder)          # several image keys: concatenated on the channel axis (agent.py:96)
         self.has_cnn = len(self.cnn_keys) > 0
         self.vec_keys = list(a.mlp_keys.encoder)
@@ -303,6 +309,9 @@ class DV3Engine:
             from sheeprl_b200.lib import CudaOps  # raises loudly if the extension / a GPU is missing
 
             ops = CudaOps(device)
+        if self.minedojo and not (hasattr(ops, "minedojo_sample") and ops.minedojo_sample_supported(actions_dim)):
+            raise NotImplementedError(f"the MineDojo actor's masked sample has no kernel for actions_dim={tuple(actions_dim)} "
+                                      f"on the {type(ops).__name__} backend")
         self.ops = ops
         self.cfg = cfg
         self.device = torch.device(device)
@@ -597,14 +606,14 @@ class DV3Engine:
             ops.increment(self.rng_t)
             ops.fill_exponential(self.noise_post.view(-1), self.rng_seed, 0, self.rng_t)
             ops.fill_exponential(self.noise_img_state.view(-1), self.rng_seed, 1, self.rng_t)
-            if self.is_continuous:
-                ops.fill_normal(self.noise_img_action.view(-1), self.rng_seed, 2, self.rng_t)
-            else:
-                ops.fill_exponential(self.noise_img_action.view(-1), self.rng_seed, 2, self.rng_t)
+            if not self.minedojo:          # the MineDojo actor imagines the mode of each head: no action noise
+                fill = ops.fill_normal if self.is_continuous else ops.fill_exponential
+                fill(self.noise_img_action.view(-1), self.rng_seed, 2, self.rng_t)
         else:
             self.noise_post.copy_(noise["post"].reshape(T, B, Z))
             self.noise_img_state.copy_(noise["img_state"].reshape(H, N, Z))
-            self.noise_img_action.copy_(torch.cat([x for x in noise["img_action"]], -1))
+            if not self.minedojo:
+                self.noise_img_action.copy_(torch.cat([x for x in noise["img_action"]], -1))
 
     def _world_model_phase(self, data: Dict[str, torch.Tensor], heads_detached: bool = False):
         """Dynamic learning (dreamer_v3.py:98-200): forward, losses, backward, clip + Adam of the world model.
@@ -1287,7 +1296,7 @@ class DV3Engine:
                 if done:
                     for k, ad in enumerate(self.actions_dim):
                         ops.head_sample(cur_in, actor.views[f"mlp_heads.{k}.weight"], actor.views[f"mlp_heads.{k}.bias"],
-                                        self.noise_img_action[i, :, off:off + ad], self.unimix,
+                                        self._img_action_noise(i, off, ad), self.unimix,
                                         self.actor_raw[rows, off:off + ad], self.actions[i, :, off:off + ad])
                         off += ad
                     continue
@@ -1299,10 +1308,15 @@ class DV3Engine:
                 continue
             off = 0
             for k, ad in enumerate(self.actions_dim):
-                ops.cat_sample(self.actor_raw[rows, off:off + ad], self.noise_img_action[i, :, off:off + ad],
+                ops.cat_sample(self.actor_raw[rows, off:off + ad], self._img_action_noise(i, off, ad),
                                self.unimix, 1, ad, self.actions[i, :, off:off + ad])
                 off += ad
 
+
+    def _img_action_noise(self, i: int, off: int, ad: int) -> Optional[torch.Tensor]:
+        """Exp(1) noise of one action head at imagination step i; None (the mode) for the MineDojo actor, whose
+        forward defaults to greedy=True when train() calls it (dreamer_v3.py:219,240; agent.py:882)"""
+        return None if self.minedojo else self.noise_img_action[i, :, off:off + ad]
 
     def _continuous_policy_gradient(self, c_logit, critics):
         """Continuous actions: objective = advantage (dreamer_v3.py:283-284), so d(policy_loss) flows from the

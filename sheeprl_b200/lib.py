@@ -389,6 +389,25 @@ class CudaOps:
         self._ck(self.lib.b200rl_head_sample(_p(X), _p(W), _p(bias), _p(noise), _p(raw), _p(onehot), M, Kin, A, _ld(X),
                                              _ld(W), _ld(raw), _ld(noise), _ld(onehot), unimix, self._st()))
 
+    def minedojo_sample_supported(self, actions_dim) -> bool:
+        return len(actions_dim) == 3 and bool(self.lib.b200rl_minedojo_sample_supported(*(int(k) for k in actions_dim)))
+
+    def minedojo_sample(self, raw, noise, unimix: float, actions_dim, onehot, mask_action_type=None,
+                        mask_craft_smelt=None, mask_equip_place=None, mask_destroy=None):
+        """onehot = MinedojoActor's masked, chained sample of the three heads [K0 | K1 | K2] of raw (noise None: the
+        mode).  Masks: float [M, K_h] rows, nonzero = allowed; None = all allowed.  One launch."""
+        _f32(raw, noise, onehot, mask_action_type, mask_craft_smelt, mask_equip_place, mask_destroy)
+        K0, K1, K2 = (int(k) for k in actions_dim)
+        M = raw.shape[0]
+        assert raw.shape == (M, K0 + K1 + K2) and onehot.shape == raw.shape, (raw.shape, onehot.shape, actions_dim)
+        assert noise is None or noise.shape == raw.shape, noise.shape
+        for mk, k in ((mask_action_type, K0), (mask_craft_smelt, K1), (mask_equip_place, K2), (mask_destroy, K2)):
+            assert mk is None or mk.shape == (M, k), (None if mk is None else mk.shape, (M, k))
+        self._ck(self.lib.b200rl_minedojo_sample(
+            _p(raw), _p(noise), _p(onehot), _p(mask_action_type), _p(mask_craft_smelt), _p(mask_equip_place),
+            _p(mask_destroy), M, K0, K1, K2, _ld(raw), _ld(noise), _ld(onehot), _ld(mask_action_type),
+            _ld(mask_craft_smelt), _ld(mask_equip_place), _ld(mask_destroy), unimix, self._st()))
+
     def cat_sample_bwd(self, raw, dz, dmix, unimix: float, groups: int, classes: int, draw):
         _f32(raw, dz, dmix, draw)
         self._ck(self.lib.b200rl_cat_sample_bwd(_p(raw), _p(dz), _p(dmix), _p(draw), raw.shape[0], groups, classes,
