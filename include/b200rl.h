@@ -319,7 +319,12 @@ int b200rl_weighted_mean(const float* x, const float* w, float* out, long long n
 
 /* ---- optimiser -----------------------------------------------------------------------------------------
  * clip_grad_norm_ + torch.optim.Adam.step fused (dreamer_v3.py:191-200,298-304,318-327); target-critic
- * EMA dreamer_v3.py:674-680; Exp(1) noise for categorical sampling (torch.multinomial). */
+ * EMA dreamer_v3.py:674-680; Exp(1) noise for categorical sampling (torch.multinomial).  The clip coefficient is
+ * clip_grad_norm_'s clamp(max_norm / (total + 1e-6), max=1): a NaN gradient element makes it NaN, and the whole group
+ * NaN, as in the reference.  sumsq (both modes), adam_step, adam_step_wd, rmsprop_step and ema are held to a float64
+ * reference with per-element first-order bounds, every step from the kernel's own state, at the float4 tails, unaligned
+ * views, several grid-stride passes, step counts up to 1e6 and non-finite gradients (tests/test_gpu_optim_precision.py),
+ * and so are copy2d, axpy, affine, symlog, tanh_fwd and tanh_bwd below. */
 int b200rl_sumsq(const float* x, long long n, double* out, cudaStream_t stream);
 int b200rl_adam_step(float* p, const float* g, float* m, float* v, const double* normsq, const int* step_dev,
                      float* norm_out, long long n, float max_norm, float lr, float b1, float b2, float eps,
@@ -331,7 +336,7 @@ int b200rl_adam_step_wd(float* p, const float* g, float* m, float* v, const doub
                         float* norm_out, long long n, float max_norm, float lr, float b1, float b2, float eps,
                         float weight_decay, cudaStream_t stream);
 /* fabric.clip_gradients + torch.optim.RMSprop.step (single-tensor path; A2C, a2c/a2c.py:102-105) in one pass, with
- * adam_step's normsq / norm_out contract.  square_avg always; momentum_buf read and written only when momentum > 0;
+ * adam_step's normsq / norm_out contract and clip coefficient.  square_avg always; momentum_buf read and written only when momentum > 0;
  * grad_avg non-NULL selects `centered`.  eps is added after the square root; the step count does not enter the update. */
 int b200rl_rmsprop_step(float* p, const float* g, float* square_avg, float* momentum_buf, float* grad_avg,
                         const double* normsq, float* norm_out, long long n, float max_norm, float lr, float alpha,
@@ -430,7 +435,8 @@ int b200rl_dropout_ln_relu_bwd(const float* dy, const float* y, const float* z, 
 /* ---- PPO --------------------------------------------------------------------------------------------------
  * Channel-last patch gather / scatter for NatureCNN's unpadded convolutions (models/models.py:288-328):
  * col[(b,oy,ox),(ky,kx,c)] = x[b,oy*s+ky,ox*s+kx,c]; col2im is its transpose (sum over overlapping patches), optionally
- * masked by ReLU'(act) of the activation that fed the convolution. */
+ * masked by ReLU'(act) of the activation that fed the convolution.  im2col is checked bit for bit and col2im against a
+ * float64 bound on the overlap sum (tests/test_gpu_optim_precision.py). */
 int b200rl_im2col(const float* x, float* col, int B, int H, int W, int C, int k, int stride, cudaStream_t stream);
 int b200rl_col2im(const float* dcol, const float* act, float* dx, int B, int H, int W, int C, int k, int stride,
                   cudaStream_t stream);

@@ -39,6 +39,13 @@ sumsq_kernel(const float* __restrict__ x, long long n, double* __restrict__ out)
   }
 }
 
+// clip_grad_norm_'s coefficient, torch.clamp(max_norm / (total + 1e-6), max=1.0): a NaN total (a NaN gradient element)
+// gives a NaN coefficient, so the whole group turns NaN as in the reference; fminf would return 1 and step unclipped.
+__device__ __forceinline__ float clip_coef(float max_norm, float total) {
+  const float c = max_norm / (total + 1e-6f);
+  return c > 1.f ? 1.f : c;
+}
+
 // WD: torch's L2 weight decay (torch/optim/adam.py: grad = grad.add(param, alpha=weight_decay)), added to the already
 // clipped gradient before the moments.  WD = false is the plain Adam kernel, so weight_decay = 0 stays bit-identical.
 template <bool WD>
@@ -49,8 +56,7 @@ adam_step_kernel(float* __restrict__ p, const float* __restrict__ g, float* __re
   __shared__ float s_coef, s_step_size, s_bc2_sqrt;
   if (threadIdx.x == 0) {
     const float total = (float)sqrt(*normsq);
-    float coef = 1.f;
-    if (max_norm > 0.f) coef = fminf(max_norm / (total + 1e-6f), 1.f);
+    const float coef = max_norm > 0.f ? clip_coef(max_norm, total) : 1.f;
     const int t = *step_t;
     const double bc1 = 1.0 - pow((double)b1, (double)t);
     const double bc2 = 1.0 - pow((double)b2, (double)t);
@@ -134,9 +140,7 @@ rmsprop_step_kernel(float* __restrict__ p, const float* __restrict__ g, float* _
   __shared__ float s_coef;
   if (threadIdx.x == 0) {
     const float total = (float)sqrt(*normsq);
-    float coef = 1.f;
-    if (max_norm > 0.f) coef = fminf(max_norm / (total + 1e-6f), 1.f);
-    s_coef = coef;
+    s_coef = max_norm > 0.f ? clip_coef(max_norm, total) : 1.f;
     if (blockIdx.x == 0) norm_out[0] = total;
   }
   __syncthreads();

@@ -27,24 +27,6 @@ def close(a, b, rtol=1e-4, atol=1e-5, what=""):
     assert bool((err <= atol + rtol * b.abs()).all()), (what, float(err.max()))
 
 
-@pytest.mark.parametrize("B,H,C,k,s", [(3, 84, 12, 8, 4), (3, 20, 32, 4, 2), (3, 9, 64, 3, 1), (2, 11, 5, 3, 2), (2, 7, 3, 7, 1)])
-def test_im2col_col2im(cu, B, H, C, k, s):
-    em = EmulOps()
-    Ho = (H - k) // s + 1
-    x = rnd(B, H, H, C, seed=1)
-    col_w = torch.zeros(B * Ho * Ho, k * k * C)
-    em.im2col(x, col_w, k, s)
-    col_g = torch.zeros_like(col_w, device="cuda")
-    cu.im2col(x.cuda(), col_g, k, s)
-    assert torch.equal(col_g.cpu(), col_w)                                # pure data movement: bit-exact
-    dcol, act = rnd(B * Ho * Ho, k * k * C, seed=2), rnd(B, H, H, C, seed=3)
-    for a in (None, act):
-        dx_w, dx_g = torch.zeros(B, H, H, C), torch.zeros(B, H, H, C, device="cuda")
-        em.col2im(dcol, a, dx_w, k, s)
-        cu.col2im(dcol.cuda(), None if a is None else a.cuda(), dx_g, k, s)
-        close(dx_g, dx_w, what="col2im")
-
-
 @pytest.mark.parametrize("cont,clipv,norm", [(False, False, False), (False, True, True), (True, False, True), (True, True, False),
                                              (2, True, True), (2, False, False)])
 def test_ppo_loss_kernel(cu, cont, clipv, norm):
